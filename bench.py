@@ -12,6 +12,7 @@ Workload: configs[2] of BASELINE.json — 4096 actors in total, sharded B/N per 
 Prints ONE JSON line (rank 0).
 """
 import argparse
+import gc
 import json
 import os
 import subprocess
@@ -27,7 +28,7 @@ UNIT = 'env-steps/s'
 TOTAL_ENVS = 4096
 T_STEPS = 50
 ACT_DIM = 18
-K1_NCU_TRAFFIC_BYTES = 32.19e6        # dram read + write of one K1 (v8) launch at B=4096 (ncu --set full, profiles/r02_k1_v8_ncu.txt)
+L2_BYTES = 50e6                       # H100 L2
 
 
 def parse():
@@ -45,11 +46,36 @@ def parse():
     ap.add_argument('--ref-deepmind-seconds', type=float, default=20.0,
                     help='--impl reference: extra run of the full wrap_deepmind pipeline flavour (0 = skip)')
     ap.add_argument('--no-pipeline', action='store_true', help='strictly sequential rollout -> learn')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the last timed step computed (rollout, learner outputs, losses, updated weights) '
+                         'as DIR/<name>.npy, so that two builds can be compared output for output')
     return ap.parse_args()
 
 
+DUMP_MAX_ELEMS = 2_000_000          # per array: the eight arrays stay within 64 MB in all
+
+
+def dump_outputs(out_dir, eng, losses, torch):
+    """The arrays a caller of the timed path receives after its last step, as float32 (float64 for the losses).
+    Arrays larger than DUMP_MAX_ELEMS are replaced by a fixed, seeded sample of their flattened elements."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    logits = eng.train_net.logits if eng.train_net is not None else eng.tgt_logits
+    values = eng.train_net.values if eng.train_net is not None else eng.values
+    arrays = dict(learner_losses=losses.double(), actions=eng.actions, rewards=eng.rewards, dones=eng.dones,
+                  behaviour_logits=eng.beh_logits, target_logits=logits, values=values,
+                  weights=torch.cat([p.detach().reshape(-1).float() for p in eng.model.parameters()]))
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32).reshape(-1)
+        if a.size > DUMP_MAX_ELEMS:
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))]
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
          'clocks_event_reasons.sw_power_cap')
@@ -93,12 +119,12 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'H100 SXM data sheet (not measured)'
 
 
 def run_reference(args, rank, world):
     """Reference arm: the reference's CPU actor-learner path (examples/IMPALA/train.py + actor.py; oracle port —
-    the Python reference itself cannot travel to the GPU box) on all host cores, learner on one B200 through torch
+    the Python reference itself is not importable here) on all host cores, learner on one GPU through torch
     eager as BASELINE.md section 3 asks.  ONE long-lived actor pool for the whole arm; a "step" is a wall-clock
     window over which sample_total_steps / elapsed is read exactly as the reference logs it (train.py:93,227,243).
     Under torchrun only rank 0 measures; the other ranks exit 0 without work."""
@@ -188,6 +214,8 @@ def main():
     import torch
     import torch.distributed as dist
     assert args.warmup >= 3, 'timing rules: at least 3 warm-up steps'
+    if args.steps < 1:
+        raise SystemExit('bench.py: --steps must be at least 1 (the timed steps)')
     if not torch.cuda.is_available():
         raise SystemExit('bench.py needs a CUDA device (no CPU fallback)')
     torch.cuda.set_device(local_rank)
@@ -234,6 +262,8 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     elapsed = elapsed_ms.item() * 1e-3
     launches = kernels.launch_count()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, losses, torch)
     # K1 bracketed by events INSIDE a step: three extra, untimed steps (no event records inside the timed region)
     k1_events = []
     eng.k1_events = k1_events
@@ -256,7 +286,7 @@ def main():
     else:
         lg, vl = eng.tgt_logits.view(T_STEPS * B, ACT_DIM), eng.values.view(-1)
     k1_args = (eng.actions.view(-1), eng.rewards.view(-1), eng.dones.view(-1), vl, T_STEPS, B, 0.99, 0.5, -0.01)
-    # (a) one event pair per launch, L2 flushed before every launch (a 256 MB fill > the 126 MB L2)
+    # (a) one event pair per launch, L2 flushed before every launch (a 256 MB fill > the 50 MB L2)
     iso = []
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     for i in range(12):
@@ -273,7 +303,7 @@ def main():
     # (b) the launch duration the roofline uses: 64 back-to-back launches over rotating copies of the logits
     # (inputs + outputs of consecutive launches never overlap; the rotation spans > 3x the L2), ONE event pair,
     # so neither the event record latency nor an L2-resident operand is in the figure
-    nrot = max(4, int(3 * 126e6 / max(1, (T_STEPS * B * ACT_DIM * 4 * 3))) + 1)
+    nrot = max(4, int(3 * L2_BYTES / max(1, (T_STEPS * B * ACT_DIM * 4 * 3))) + 1)
     rot = [(lg.clone(), eng.beh_logits.view(T_STEPS * B, ACT_DIM).clone(),
             dict(losses=torch.zeros(8, device=dev), d_logits=torch.empty((T_STEPS * B, ACT_DIM), device=dev),
                  d_values=torch.empty(T_STEPS * B, device=dev))) for _ in range(nrot)]
@@ -321,20 +351,15 @@ def main():
     roof = None
     if k1_s:
         ach = alg_bytes / k1_s / 1e9
-        # traffic: dram__bytes_read.sum + dram__bytes_write.sum of one launch at B=4096 from the committed
-        # `ncu --set full` capture of this kernel version (profiles/r02_k1_v8_ncu.txt); the gradient tile (15.3 MB) is
-        # mostly still in the 126 MB L2 when the launch ends, so the write half shows up only partly
-        traffic = K1_NCU_TRAFFIC_BYTES if B == 4096 else None
         roof = dict(bound='hbm', kernel='vtrace_loss_v8_kernel (rl_vtrace_loss_fwd_bwd)', achieved=ach, peak=peak,
-                    unit='GB/s', frac=ach / peak, traffic=traffic, peak_source=peak_src,
+                    unit='GB/s', frac=ach / peak, peak_source=peak_src,
                     algorithmic_bytes_per_launch=alg_bytes, us_per_launch=k1_s * 1e6,
                     us_per_launch_l2_flushed_single_event_pair=k1_flushed_s * 1e6,
                     frac_l2_flushed_single_event_pair=alg_bytes / k1_flushed_s / 1e9 / peak,
                     us_per_launch_in_pipelined_step=k1_in_step_us,
                     l2='%d rotating operand sets (> 3x L2), %s, one event pair per replay, median of 5' % (nrot, k1_timing))
 
-    # the kernel with the largest share of the step (profiles/r01_bench_launches_final.txt: 15 %): conv1 forward in
-    # TMA-window form, timed here live at the learner's batch on the step's own buffers (11.6 GB in, 7.5 GB out: far
+    # conv1 forward in TMA-window form, timed here live at the learner's batch on the step's own buffers (11.6 GB in, 7.5 GB out: far
     # beyond L2, nothing to flush), CUDA events on the launching stream, nothing else in flight
     dom = None
     try:
@@ -349,10 +374,10 @@ def main():
         pk = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
         tpeak, tsrc = float(pk['bf16_tflops_sustained']), 'measured (MEASURED_PEAKS.json bf16_tflops_sustained)'
     except Exception:
-        tpeak, tsrc = 1400.0, 'fallback (B200_PROFILING.md sustained)'
+        tpeak, tsrc = 989.0, 'H100 SXM data sheet, dense BF16 (not measured)'
     flops_per_step = 4 * 25.8e6 * T_STEPS * B
     ach_tf = flops_per_step * args.steps / elapsed / 1e12
-    net_roof = dict(bound='tensor', what='policy/value network (tcgen05 conv/GEMM kernels), per GPU', achieved=ach_tf,
+    net_roof = dict(bound='tensor', what='policy/value network (wgmma conv/GEMM kernels), per GPU', achieved=ach_tf,
                     peak=tpeak, unit='TFLOP/s', frac=ach_tf / tpeak, peak_source=tsrc)
 
     # HBM view of the whole step: with the convolutions at 2x2/3x3 filters on 32..128 channels the network kernels are
@@ -370,9 +395,17 @@ def main():
                      achieved=ach_hbm, peak=peak, unit='GB/s', frac=ach_hbm / peak, peak_source=peak_src,
                      algorithmic_bytes_per_env_step=per_env_step) if eng.train_net is not None else None
 
+    pipelined, net_native = eng.pipeline, eng.train_net is not None
+    obs_gb = T_STEPS * B * 28224 * eng.obs_step.element_size() / 1e9
     e2e = None
     if not args.no_e2e:
-        e2e = run_e2e(eng, args, world, dev)
+        # the host-contract path builds its own actor pool and learner: release this engine first so that both
+        # fit in the 80 GB of one H100
+        del eng, lg, vl, k1_args
+        gc.collect()
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()
+        e2e = run_e2e(args, world, dev)
     cpu = None
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         cpu = cpu_baseline_subprocess(args)
@@ -385,13 +418,13 @@ def main():
                                 envs_per_gpu=B, T=T_STEPS, learner_batch=T_STEPS * args.envs,
                                 model='84x84 actor-critic (benchmark/torch/a2c/atari_model.py), 2.74 M params',
                                 parallelism='dp%d' % world,
-                                actor_learner='pipelined (rollout k+1 || learn k, policy lag 1)' if eng.pipeline
+                                actor_learner='pipelined (rollout k+1 || learn k, policy lag 1)' if pipelined
                                 else 'sequential',
-                                network='hand-written tcgen05 kernels (actor fwd; learner fwd+dgrad+wgrad)' if
-                                eng.train_net is not None else 'torch',
+                                network='hand-written wgmma kernels (actor fwd; learner fwd+dgrad+wgrad)' if
+                                net_native else 'torch',
                                 l2_policy='per-step working set (frame ring %.1f GB + observation plane %.1f GB + '
-                                          'activations %.1f GB per GPU) >> 126 MB L2; K1 timed alone with L2 flushed' %
-                                          ((T_STEPS + 4) * B * 7056 / 1e9, T_STEPS * B * 28224 * eng.obs_step.element_size() / 1e9,
+                                          'activations %.1f GB per GPU) >> 50 MB L2; K1 timed alone with L2 flushed' %
+                                          ((T_STEPS + 4) * B * 7056 / 1e9, obs_gb,
                                            T_STEPS * B * 120e3 / 1e9)),
                     gpu_launches=launches, clocks=clocks, roofline=dom if dom is not None else roof, roofline_k1=roof,
                     roofline_network=net_roof, roofline_step=step_roof,
@@ -401,12 +434,6 @@ def main():
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
-
-
-# dram__bytes_read.sum + dram__bytes_write.sum per sample of conv1 forward from the committed ncu captures:
-# bf16 input (profiles/r01_learner_kernels_final.txt: 2.948 GB + 1.282 GB at 51 200 samples); uint8 input
-# (profiles/r02_conv1_u8_ncu.txt: 1.445 GB + 1.270 GB)
-CONV1_NCU_TRAFFIC_PER_SAMPLE = {False: (2.947656e9 + 1.281806e9) / 51200.0, True: (1.445169e9 + 1.269890e9) / 51200.0}
 
 
 def measure_dominant_kernel(eng, kernels, torch, B, peak, peak_src):
@@ -435,17 +462,14 @@ def measure_dominant_kernel(eng, kernels, torch, B, peak, peak_src):
     in_bytes = 21 * 21 * 64 * (1 if u8 else 2)
     alg_bytes = n * (4 * 84 * 84 + 20 * 20 * 32 * 2)
     ach = alg_bytes / sec / 1e9
-    # traffic: dram__bytes_read.sum + dram__bytes_write.sum of this kernel in the committed `ncu --set full` capture
-    # (CONV1_NCU_TRAFFIC: bytes per sample), scaled to this launch's samples
-    traffic = CONV1_NCU_TRAFFIC_PER_SAMPLE[u8] * n if CONV1_NCU_TRAFFIC_PER_SAMPLE[u8] else None
     name = 'shiftconv_fwd_kernel<32,1,2,0,%s> (%s, conv1 forward at the learner batch)' % (
         'true' if u8 else 'false', 'rl_conv2d_s1_u8in_bf16_fwd' if u8 else 'rl_conv2d_s1_nhwc_bf16_fwd')
     return dict(bound='hbm', kernel=name,
-                achieved=ach, peak=peak, unit='GB/s', frac=ach / peak, traffic=traffic, peak_source=peak_src,
+                achieved=ach, peak=peak, unit='GB/s', frac=ach / peak, peak_source=peak_src,
                 algorithmic_bytes_per_launch=alg_bytes, us_per_launch=sec * 1e6, samples_per_launch=n,
                 bytes_moved_per_launch_as_built=n * (in_bytes + 20 * 20 * 32 * 2),
                 frac_of_peak_as_built=n * (in_bytes + 20 * 20 * 32 * 2) / sec / 1e9 / peak,
-                l2='operands (%.1f GB + 7.5 GB at 204 800 samples) far beyond the 126 MB L2' % (204800 * in_bytes / 1e9))
+                l2='operands (%.1f GB + 7.5 GB at 204 800 samples) far beyond the 50 MB L2' % (204800 * in_bytes / 1e9))
 
 
 def numa_pin(gpu_index):
@@ -508,7 +532,7 @@ def copy_bandwidth_bidir(torch, dev, nbytes=1 << 30):
                 d2h=reps * nbytes / (ev[2].elapsed_time(ev[3]) * 1e-3) / 1e9)
 
 
-def run_e2e(eng, args, world, dev):
+def run_e2e(args, world, dev):
     """The same metric END TO END through the reference-facing surface with HOST buffers, exactly the Learner loop of
     examples/IMPALA/train.py:165-194: a ``@parl.remote_class(wait=False)`` Actor (the device actor pool) whose
     ``sample()`` returns the numpy sample dict (uint8 stacked obs, env-major; D2H into pinned memory inside the
@@ -530,7 +554,7 @@ def run_e2e(eng, args, world, dev):
     if world > 1:
         agent.alg.grad_sync = lambda g: dist.all_reduce(g, op=dist.ReduceOp.SUM)
     actor = Actor(cfg, device=dev)
-    steps = max(10, min(args.steps, 20))
+    steps = args.steps
     actor.set_weights(agent.get_weights()).get()
     fut = actor.sample()
 

@@ -1,7 +1,7 @@
 """IMPALA training script in the shape of the reference's examples/IMPALA/train.py (Learner with sampling threads, a
 bounded sample queue, a learn thread, stale parameter broadcast, schedulers, WindowStat / TimeStat metrics) running on
 parl_b200: the remote Actor is the DEVICE actor pool (one actor = thousands of lock-stepped envs on the GPU) and the
-agent's learn() is the tcgen05 learner.  Only the imports differ from a reference-style script:
+agent's learn() is the wgmma learner.  Only the imports differ from a reference-style script:
 
     import parl_b200; parl_b200.install_as_parl()      # then: import parl ... exactly as with PaddlePaddle/PARL
 

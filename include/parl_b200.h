@@ -1,5 +1,5 @@
 /*
- * parl_b200 — C ABI of the B200 (sm_100a) actor-learner hot path.
+ * parl_b200 — C ABI of the H100 (sm_90a) actor-learner hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b): plain pointers and sizes, no
  * torch / C++ types.  Every entry point names the PaddlePaddle/PARL code whose
@@ -58,14 +58,14 @@ size_t rl_loss_workspace_bytes(int n_cols);
  * TMA tensor-map path run when the layout allows it. */
 /* 1: the per-env-step chain kernels (observation gather, TMA-window convs, GEMMs, env step) are launched with
  * programmatic stream serialization: each starts its prologue while the previous kernel of the stream drains and
- * blocks on griddepcontrol.wait before touching dependent memory.  0 (default): plain stream order — measured equal
- * for the graph-replayed rollout and slower for the pipelined step (profiles/r02_pdl_ab.txt). */
+ * blocks on griddepcontrol.wait before touching dependent memory.  0 (default): plain stream order (early-resident
+ * CTAs would hold SMs the other stream of a pipelined step could use; not measured on H100). */
 int rl_debug_set_pdl(int enable);
 int rl_debug_set_tma(int disable);
 /* Triage hook for rl_vtrace_loss_fwd_bwd: 0 = default (the v8 kernel for time-major, TMA-able shapes with T <= 64,
  * B % 4 == 0, even A <= 18 and int32 actions; the general v4 kernel otherwise), 4 = v4 always, 8 / 9 = v8 without /
- * with programmatic dependent launch (measured equal: profiles/r02_k1_matrix_g.jsonl), 10 / 11 = v8 with 256-byte / no L2
- * promotion in the logits tensor maps (no effect: profiles/r02_k1_l2_promotion.jsonl). */
+ * with programmatic dependent launch, 10 / 11 = v8 with 256-byte / no L2 promotion in the logits tensor maps (128 B is
+ * the default). */
 int rl_debug_set_vtrace_path(int mode);
 
 /* ------------------------------------------------------------------------
@@ -341,15 +341,14 @@ int rl_adam_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq, l
 int rl_gather_cast(const float* src, const int32_t* idx, long long n, void* out, int out_bf16, rl_stream_t stream);
 
 /* ------------------------------------------------------------------------
- * a13 / K6  Dense contraction on the tcgen05 tensor cores (TMA-staged tiles, fp32 accumulation in TMEM):
+ * a13 / K6  Dense contraction on the Hopper tensor cores (TMA-staged tiles, wgmma with fp32 register accumulators):
  *   C[M,N] = act(A[M,K] . B[N,K]^T + bias[N])      A, B bf16 row-major ("x . W^T"), C bf16 or f32.
  * Replaces the nn.Linear forward of the reference models (e.g. benchmark/torch/a2c/atari_model.py:46-49,
  * executed there by cuBLAS through torch).  lda/ldb/ldc in elements; lda, ldb multiples of 8.
  * ---------------------------------------------------------------------- */
 int rl_gemm_bf16_tn(const void* A, const void* B, const float* bias, void* C, int M, int N, int K,
                     int lda, int ldb, int ldc, int relu, int out_f32, rl_stream_t stream);
-/* 1 (default): outputs of at least 2 x 2 tiles of width >= 128 run as 2 x 2 thread-block clusters whose CTAs multicast
- * their operand half-tiles to each other (each operand byte leaves L2 once per cluster); 0: single-CTA form only. */
+/* GEMM tile form: 0 (the only form built for sm_90a) = single-CTA tiles; anything else is rejected. */
 int rl_debug_set_gemm_cluster(int enable);
 /* Hidden layer + small heads in one call (the actor's fc 5184->512 followed by the policy head,
  * benchmark/torch/a2c/atari_model.py:46-49,60-66): H = act(A.B^T + bias) [M,N] bf16 as rl_gemm_bf16_tn(_splitk), then
@@ -375,7 +374,7 @@ int rl_gemm_bf16_tn_splitk(const void* A, const void* B, const float* bias, void
 int rl_gemm_bf16_tn_masked(const void* A, const void* B, void* C, const void* mask, int M, int N, int K,
                            int lda, int ldb, int ldc, int ldm, int out_f32, rl_stream_t stream);
 
-/* NHWC bf16 convolution forward (+bias, optional ReLU) as an implicit GEMM on tcgen05: the conv layers of
+/* NHWC bf16 convolution forward (+bias, optional ReLU) as an implicit GEMM on the tensor cores (wgmma): the conv layers of
  * the Atari actor-critic (benchmark/torch/a2c/atari_model.py:26-44; executed there by cuDNN through torch).
  *   in [N,Hin,Win,Cin] bf16, weight_krsc [Cout, KH*KW*Cin] bf16 with K ordered (r, s, c), bias [Cout] f32,
  *   out [N,Hout,Wout,Cout] bf16.  Cin, Cout in {32, 64}; KH*KW*Cin a multiple of 64. */
@@ -385,7 +384,7 @@ int rl_conv2d_nhwc_bf16_fwd(const void* in, const void* weight_krsc, const float
 
 /* Stride-1 NHWC bf16 convolution forward in TMA-window form (no operand gather): a conv over the flattened
  * pixel sequence is a sum of shifted GEMMs; one TMA load per 128-position tile brings the input window into
- * shared memory and every filter tap is a tcgen05.mma whose descriptor starts (r*W+s) rows further down.
+ * shared memory and every filter tap is a wgmma whose descriptor starts (r*W+s) rows further down.
  * Stride-2/4 layers use it through space-to-depth of their input.  in [N,H,W,Cin], weight [Cout, KH*KW*Cin]
  * ordered (r,s,c); out_mode 0: out [N,H-KH+1,W-KW+1,Cout]; out_mode 1 (20x20 outputs only): out is the
  * zero-padded 2x2 space-to-depth tensor [N,12,12,4*Cout] that feeds a following 4x4/stride-2/pad-2 conv.
@@ -394,12 +393,12 @@ int rl_conv2d_s1_nhwc_bf16_fwd(const void* in, const void* weight_krsc, const fl
                                int N, int H, int W, int Cin, int Cout, int KH, int KW, int relu, int out_mode,
                                rl_stream_t stream);
 int rl_debug_set_shiftconv_base_offset(int enable);
-/* 0 (default): one MMA group per filter tap; 1: column-tap-fused tile (the KW taps of a filter row share one
- * A-operand read, N' = KW*Cout accumulator columns, shifted sum in the epilogue) — measured slower on B200, kept as
- * an experiment and cross-check. */
+/* Tile form of the window conv: 0 (default) = one MMA chain per filter tap, the tap shift applied to the operand
+ * window; 1 = per filter column, the column shift applied to the output rows through a shared-memory fp32 tile
+ * (a cross-check of the tap / shift bookkeeping). */
 int rl_debug_set_shiftconv_form(int form);
 /* The same forward for conv1 of the Atari models on the uint8 observation: in_u8 [N,H,W,64] uint8 (space-to-depth,
- * rl_obs_stack_gather out_dtype 4); operand = bf16(byte * in_scale), converted in shared memory by four extra warps,
+ * rl_obs_stack_gather out_dtype 4); operand = bf16(byte * in_scale), converted in shared memory by 256 extra threads,
  * bit-identical to feeding rl_conv2d_s1_nhwc_bf16_fwd the out_dtype-3 tensor at half the input traffic.
  * Built for KH = KW = 2, Cin = 64, Cout = 32. */
 int rl_conv2d_s1_u8in_bf16_fwd(const void* in_u8, float in_scale, const void* weight_krsc, const float* bias, void* out,
@@ -417,12 +416,12 @@ int rl_conv2d_s1_nhwc_bf16_dgrad(const void* dout_grid, const void* weight_t_krs
                                  int OGH, int OGW, rl_stream_t stream);
 
 /* Weight gradient of rl_conv2d_s1_nhwc_bf16_fwd in TMA-window form: dW[co][(r,s,ci)] = sum_q dout_grid[q,co] *
- * in[q + r*W + s, ci] with the position index as the GEMM reduction dimension (tcgen05, MN-major operands,
- * accumulators resident in TMEM over the CTA's whole position range, deterministic two-stage reduction).
+ * in[q + r*W + s, ci] with the position index as the GEMM reduction dimension (wgmma, MN-major operands,
+ * accumulators resident in registers over the CTA's whole position range, deterministic two-stage reduction).
  * dout_grid [N,H,W,Cout] on the input grid (zeros at invalid positions), in [N,H,W,Cin], dw_krsc [Cout, KH*KW*Cin]
- * float32 (accumulate=1 adds to it).  (Cout, Cin) = (64, 64|128), or (32, 64) where the 64-byte dout rows are the
- * SWIZZLE_64B N-operand of a role-swapped product.  db (optional, [Cout] float32) receives the bias gradient
- * sum_q dout_grid[q, :] from the same pass (one extra tcgen05.mma per K step against a tile of ones).
+ * float32 (accumulate=1 adds to it).  (Cout, Cin) = (64, 64|128), or (32, 64) where the 64-byte dout rows are a
+ * SWIZZLE_64B operand.  db (optional, [Cout] float32) receives the bias gradient
+ * sum_q dout_grid[q, :] from the same pass (one extra wgmma per K step against a tile of ones).
  * Workspace: rl_conv_wgrad_workspace_bytes. */
 size_t rl_conv_wgrad_workspace_bytes(int KH, int KW, int Cin);
 int rl_conv2d_s1_nhwc_bf16_wgrad(const void* dout_grid, const void* in, float* dw_krsc, float* db, int N, int H, int W,
@@ -432,6 +431,8 @@ int rl_conv2d_s1_nhwc_bf16_wgrad(const void* dout_grid, const void* in, float* d
 int rl_conv2d_s1_u8in_bf16_wgrad(const void* dout_grid, const void* in_u8, float in_scale, float* dw_krsc, float* db,
                                  int N, int H, int W, int Cout, int KH, int KW, int accumulate,
                                  void* workspace, size_t workspace_bytes, rl_stream_t stream);
+/* Weight-gradient form: 0 (default) = A = input window, B = dout, bias gradient in the same pass; 2 = for Cout = 64
+ * the operand roles swapped and the bias gradient by rl_colsum_bf16 (accumulate with db is then rejected). */
 int rl_debug_set_wgrad_lane_map(int mode);
 /* out[c] = sum_r x[r,c] for a [rows, C] bf16 matrix (bias gradients); C a multiple of 8 with C/8 dividing 256;
  * workspace >= 1184*C*4 bytes. */

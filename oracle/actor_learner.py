@@ -21,7 +21,7 @@ Actors are OS processes (one per core, single-threaded torch, as the reference's
 parl/core/torch/agent.py:26, parl/remote/job.py:17) forked ONCE per cluster; they ship their sample dict
 back by pickle over a pipe (standing in for cloudpickle + ZeroMQ, parl/remote/communication.py:59-130).
 The learner is torch eager float32 on one CUDA device when one is present (BASELINE.md section 3: "learner on
-one B200 via torch eager"), else on the CPU threads the actors leave.  paddle is absent, so the network is the
+one H100 via torch eager"), else on the CPU threads the actors leave.  paddle is absent, so the network is the
 torch twin of the C3 model and V-trace is the reference's Python loop over T (vtrace.py:116-122) in torch.
 Used only by bench.py (cpu_baseline / --impl reference) and tests.
 """

@@ -1,9 +1,9 @@
-"""parl_b200 — a B200-native actor-learner RL engine behind PaddlePaddle/PARL's API.
+"""parl_b200 — a H100-native actor-learner RL engine behind PaddlePaddle/PARL's API.
 
 Keeps ``parl.Model / Algorithm / Agent``, ``parl.algorithms.{IMPALA,A2C,PPO,DQN,DDQN,PolicyGradient}``
 and the ``parl.remote_class`` / ``parl.connect`` decorator surface; the hot path (vectorised env
 stepping, action sampling, return scans, losses and their gradients, clip + Adam) runs in
-hand-written sm_100a kernels behind the C ABI of include/parl_b200.h.
+hand-written sm_90a kernels behind the C ABI of include/parl_b200.h.
 
 ``import parl_b200 as parl`` or ``parl_b200.install_as_parl()`` (then ``import parl`` resolves here).
 """

@@ -23,7 +23,7 @@ def ensure_cuda(model, name):
     dev = model_device(model)
     if dev.type != 'cuda':
         if not torch.cuda.is_available():
-            raise RuntimeError('%s: parl_b200 algorithms run on the B200 only (no CPU fallback) and no CUDA '
+            raise RuntimeError('%s: parl_b200 algorithms run on the H100 only (no CPU fallback) and no CUDA '
                                'device is visible' % name)
         model.to(torch.device('cuda', torch.cuda.current_device()))
         dev = model_device(model)

@@ -1,4 +1,4 @@
-"""Build libparl_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libparl_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m parl_b200.build [--force] [-v]
 
@@ -15,8 +15,9 @@ from concurrent.futures import ThreadPoolExecutor
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'csrc')
 LIB = os.path.join(CSRC, 'libparl_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
-         '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17',
+        '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
 def _sources():
@@ -59,7 +60,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    cmd = [NVCC, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs
+    cmd = [NVCC, '-shared'] + ARCH + ['-o', LIB] + objs
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

@@ -1,6 +1,6 @@
 """``parl.Model`` on PyTorch — host-side mirror of parl/core/torch/model.py:24-134.
 
-Parameters stay torch tensors (on the B200); ``get_weights`` / ``set_weights`` keep the
+Parameters stay torch tensors (on the H100); ``get_weights`` / ``set_weights`` keep the
 reference's numpy-dict contract (one entry per ``state_dict`` key, in order) and
 ``sync_weights_to`` keeps ``target = decay*target + (1-decay)*self``
 (behaviours pinned by parl/core/torch/tests/model_base_test_torch.py:53-335).

@@ -17,10 +17,7 @@ void set_error(const char* fmt, ...) {
 static int g_sm_limit = 0;
 int effective_sms(int sms) { return (g_sm_limit > 0 && g_sm_limit < sms) ? g_sm_limit : sms; }
 // Programmatic dependent launch of the actor-chain kernels (common.cuh: launch_chain / pdl_wait).  OFF by default:
-// measured on B200 (profiles/r02_pdl_ab.txt) the graph-replayed rollout does not get shorter (2.80 vs 2.78 ms at 512
-// envs: the replayed launches are already back to back and the prologues are short) and the pipelined step gets
-// LONGER (6.12 vs 5.29 ms at 512 envs, 36.6 vs 35.9 ms at 4096): early-resident CTAs of the next kernel hold SMs that
-// the other stream's kernels could have used.
+// early-resident CTAs of the next kernel hold SMs that the other stream's kernels of a pipelined step could use.
 static int g_pdl = 0;
 int pdl_enabled() { return g_pdl; }
 }  // namespace rl

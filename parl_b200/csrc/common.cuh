@@ -1,4 +1,4 @@
-// Shared device/host helpers for the parl_b200 kernels (sm_100a only).
+// Shared device/host helpers for the parl_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -56,7 +56,7 @@ static inline void opt_in_max_dynamic_smem(Kernel kernel, unsigned long long* do
 
 #ifdef __CUDACC__
 // Programmatic dependent launch (actor chain: 7 short kernels per env step).  A kernel launched through launch_chain
-// may begin while its predecessor in the stream is still draining: its prologue (barrier init, TMEM allocation,
+// may begin while its predecessor in the stream is still draining: its prologue (barrier init,
 // tensor-map prefetch, weight loads — nothing a predecessor writes) runs ahead, pdl_wait() then blocks until the
 // predecessor grid has completed and its writes are visible, and pdl_trigger() lets the NEXT kernel in the stream start
 // its own prologue.  Every kernel launched this way MUST call pdl_wait() before its first access to memory another

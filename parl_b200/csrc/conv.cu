@@ -1,84 +1,32 @@
-// K6 (convolutions) — NHWC bf16 convolution forward as an implicit GEMM on the tcgen05 tensor cores:
+// K6 (convolutions) — NHWC bf16 convolution forward as an implicit GEMM on the Hopper tensor cores:
 //   out[n,oh,ow,:] = relu( sum_{r,s,c} in[n, oh*stride-pad+r, ow*stride-pad+s, c] * W[:, (r,s,c)] + bias )
 // for the three conv layers of the Atari actor-critic (a13: benchmark/torch/a2c/atari_model.py:26-44; conv1
 // in its space-to-depth form, see rl_obs_stack_gather out_dtype 3).  GEMM view: M = N*Hout*Wout output
 // pixels, N = Cout (32 / 64), K = KH*KW*Cin ordered (r, s, c) so that one 128-byte k-block is 1 or 2 filter taps.
 //
-// sm_100a structure (persistent CTAs, one per SM, tiles of 128 output pixels):
-//   warps 0-3 : producers — thread i gathers row i of the 128 x 64 A k-block straight from the NHWC input with
-//               16-byte cp.async (zero-fill outside the image), writing the SWIZZLE_128B K-major layout by hand;
-//               a kStages-deep ring, completion published per stage through "full" mbarriers
-//   warp 4    : weights [Cout, K] stay RESIDENT in shared memory (one TMA load per CTA); one elected thread
-//               issues tcgen05.mma (M=128, N=Cout, K=16) into a double-buffered TMEM accumulator
-//   warps 5-8 : epilogue — tcgen05.ld, bias + ReLU, bf16 pack, one contiguous Cout*2-byte row store per pixel
-// Tensor-pipe bound (2*M*Cout*K flops); with Cout <= 64 the shared-memory A-operand bandwidth caps the MMA
-// rate at roughly half of peak (B300_MICROARCH.md: SS-mode operand reads).
+// sm_90a structure (persistent CTAs, one per SM, tiles of 128 output pixels):
+//   warps 0-3      : producers — thread i gathers row i of the 128 x 64 A k-block straight from the NHWC input with
+//                    16-byte cp.async (zero-fill outside the image), writing the SWIZZLE_128B K-major layout by hand;
+//                    a kStages-deep ring, completion published per stage through "full" mbarriers
+//   warpgroups 1-2 : weights [Cout, K] stay RESIDENT in shared memory (one TMA load per CTA); warpgroup c issues
+//                    wgmma m64nCout for rows [64c, 64c + 64) of each tile, then bias + ReLU, bf16, NHWC store
+//                    straight from its accumulator registers
 #include <cuda_bf16.h>
 
 #include "common.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace rl {
 
-// ---- tcgen05 wrappers (same encodings as gemm.cu) -----------------------------------------------
-__device__ __forceinline__ void c_tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void c_tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void c_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void c_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void c_umma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void c_commit(void* mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(mbar))
-               : "memory");
-}
-__device__ __forceinline__ void c_tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ uint64_t c_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t c_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 __device__ __forceinline__ void cp_async16_zfill(uint32_t smem_dst, const void* gsrc, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(smem_dst), "l"(gsrc), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(void* mbar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(mbar)) : "memory");
 }
 
 constexpr int kCvBM = 128;
 constexpr int kCvStages = 6;
 constexpr int kCvLag = 3;            // cp.async groups in flight per producer thread before publishing a stage
-constexpr int kCvThreads = 288;      // 4 producer warps + 1 MMA warp + 4 epilogue warps
+constexpr int kCvThreads = 384;      // 4 producer warps + 2 consumer warpgroups
 
 struct ConvArgs {
   const __nv_bfloat16* in;   // [N, Hin, Win, Cin]
@@ -93,36 +41,25 @@ __global__ void __launch_bounds__(kCvThreads, 1) conv_igemm_fwd_kernel(const __g
                                                                        const ConvArgs g) {
   constexpr int A_STAGE = kCvBM * 128;          // 16 KB: 128 rows x 64 bf16
   constexpr int W_KB = COUT * 128;              // bytes of one weight k-block
-  constexpr int TMEM_COLS = 2 * COUT < 32 ? 32 : 2 * COUT;
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   unsigned char* sW = smem;                                    // [num_kb][COUT][128 B]
   unsigned char* sA = smem + ((g.num_kb * W_KB + 1023) & ~1023);   // [stages][128][128 B]
-  __shared__ __align__(8) unsigned long long full_bar[kCvStages], empty_bar[kCvStages], w_bar, tmem_full[2], tmem_empty[2];
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) unsigned long long full_bar[kCvStages], empty_bar[kCvStages], w_bar;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_w);
     for (int s = 0; s < kCvStages; ++s) {
       mbar_init(&full_bar[s], 128);              // every producer thread arrives
-      mbar_init(&empty_bar[s], 1);               // tcgen05.commit
+      mbar_init(&empty_bar[s], 2);               // one arrival per consumer warpgroup
     }
     mbar_init(&w_bar, 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full[b], 1);               // tcgen05.commit
-      mbar_init(&tmem_empty[b], 128);            // every epilogue thread arrives
-    }
     fence_mbar_init();
   }
-  if (warp == 4) c_tmem_alloc(&tmem_base_smem, TMEM_COLS);
-  c_fence_before();
   __syncthreads();
-  c_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   const int HWo = g.Hout * g.Wout;
 
-  if (warp < 4) {
+  if (threadIdx.x < 128) {
     // ===================== producers: implicit-GEMM gather of the A operand =====================
     const int row = threadIdx.x;                                   // 0..127
     const uint32_t row_smem = (uint32_t)row * 128u;
@@ -173,67 +110,47 @@ __global__ void __launch_bounds__(kCvThreads, 1) conv_igemm_fwd_kernel(const __g
     cp_async_wait<0>();
     fence_proxy_async_smem();
     for (uint32_t d = (it >= (uint32_t)kCvLag ? it - kCvLag : 0u); d < it; ++d) mbar_arrive(&full_bar[d % kCvStages]);
-  } else if (warp == 4) {
-    // ===================== weights (once) + MMA issue =====================
-    if (lane == 0) {
-      mbar_arrive_expect_tx(&w_bar, (uint32_t)(g.num_kb * W_KB));
-      for (int kb = 0; kb < g.num_kb; ++kb) tma_load_2d(sW + kb * W_KB, &map_w, kb * 64, 0, &w_bar);
-      mbar_wait(&w_bar, 0);
-      constexpr uint32_t idesc = c_idesc_bf16(kCvBM, COUT);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++tcount) {
-        const uint32_t buf = tcount & 1u;
-        mbar_wait(&tmem_empty[buf], ((tcount >> 1) & 1u) ^ 1u);   // epilogue has drained this accumulator
-        c_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * COUT;
-        for (int kb = 0; kb < g.num_kb; ++kb, ++it) {
-          const uint32_t s = it % kCvStages;
-          mbar_wait(&full_bar[s], (it / kCvStages) & 1u);
-          c_fence_after();
-          const uint64_t da = c_desc_sw128(smem_u32(sA + s * A_STAGE));
-          const uint64_t db = c_desc_sw128(smem_u32(sW + kb * W_KB));
+    return;
+  }
+  // ===================== consumers: weights (once), wgmma, epilogue =====================
+  const int c = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127;
+  if (threadIdx.x == 128) {
+    mbar_arrive_expect_tx(&w_bar, (uint32_t)(g.num_kb * W_KB));
+    for (int kb = 0; kb < g.num_kb; ++kb) tma_load_2d(sW + kb * W_KB, &map_w, kb * 64, 0, &w_bar);
+  }
+  mbar_wait(&w_bar, 0);
+  const uint32_t a_lo0 = gmma_lo(sA) + (uint32_t)(c * 64 * 128 >> 4), w_lo0 = gmma_lo(sW);
+  float bias_r[COUT / 2];                      // bias of the column of each accumulator element
 #pragma unroll
-          for (int k = 0; k < 4; ++k) c_umma(d_tmem, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
-          c_commit(&empty_bar[s]);
-        }
-        c_commit(&tmem_full[buf]);
-      }
+  for (int i = 0; i < COUT / 2; ++i) bias_r[i] = __ldg(g.bias + gmma_col(t, i));
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
+    float d[COUT / 2];
+#pragma unroll
+    for (int i = 0; i < COUT / 2; ++i) d[i] = 0.f;
+    for (int kb = 0; kb < g.num_kb; ++kb, ++it) {
+      const uint32_t s = it % kCvStages;
+      mbar_wait(&full_bar[s], (it / kCvStages) & 1u);
+      wgmma_fence();
+      const uint32_t a_lo = a_lo0 + s * (uint32_t)(A_STAGE >> 4), w_lo = w_lo0 + (uint32_t)(kb * (W_KB >> 4));
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_bf16<COUT>(d, gmma_desc(kGmmaHiSw128, a_lo + 2 * k), gmma_desc(kGmmaHiSw128, w_lo + 2 * k), (kb | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (t == 0) mbar_arrive(&empty_bar[s]);
     }
-  } else {
-    // ===================== epilogue: TMEM -> bias + ReLU -> bf16 NHWC rows =====================
-    const int q = warp & 3;
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++tcount) {
-      const uint32_t buf = tcount & 1u;
-      mbar_wait(&tmem_full[buf], (tcount >> 1) & 1u);
-      c_fence_after();
-      const int m = tile * kCvBM + q * 32 + lane;
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * COUT;
+    wgmma_fence_regs(d);
 #pragma unroll
-      for (int c0 = 0; c0 < COUT; c0 += 16) {
-        float v[16];
-        c_tmem_ld16(taddr + (uint32_t)c0, v);
-        if (m < g.M) {
-          uint32_t pk[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float x0 = v[2 * i] + __ldg(g.bias + c0 + 2 * i), x1 = v[2 * i + 1] + __ldg(g.bias + c0 + 2 * i + 1);
-            if (g.relu) x0 = fmaxf(x0, 0.f), x1 = fmaxf(x1, 0.f);
-            __nv_bfloat162 h = __floats2bfloat162_rn(x0, x1);
-            pk[i] = *reinterpret_cast<uint32_t*>(&h);
-          }
-          uint4* dst = reinterpret_cast<uint4*>(g.out + (size_t)m * COUT + c0);
-          dst[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          dst[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-        }
+    for (int i = 0; i < COUT / 2; i += 2) {
+      const int m = tile * kCvBM + 64 * c + gmma_row(t, i), col = gmma_col(t, i);
+      if (m < g.M) {
+        float x0 = d[i] + bias_r[i], x1 = d[i + 1] + bias_r[i + 1];
+        if (g.relu) x0 = fmaxf(x0, 0.f), x1 = fmaxf(x1, 0.f);
+        *reinterpret_cast<__nv_bfloat162*>(g.out + (size_t)m * COUT + col) = __floats2bfloat162_rn(x0, x1);
       }
-      c_fence_before();
-      mbar_arrive(&tmem_empty[buf]);
     }
   }
-  c_fence_before();
-  __syncthreads();
-  if (warp == 4) c_tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 static int make_weight_map(CUtensorMap* map, const void* w, int K, int Cout) {
@@ -294,7 +211,7 @@ extern "C" int rl_conv2d_nhwc_bf16_fwd(const void* in, const void* weight_krsc, 
     set_error("conv2d_nhwc_bf16_fwd: cuTensorMapEncodeTiled failed");
     return RL_ERR_CUDA;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   cudaStream_t st = (cudaStream_t)stream;

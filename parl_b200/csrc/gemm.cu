@@ -1,20 +1,20 @@
-// K6 (dense contractions) — bf16 GEMM on the 5th-gen tensor cores: C[M,N] = act(A[M,K] · B[N,K]^T + bias)
-// with fp32 accumulation in TMEM.  Used for the linear layers of the policy/value networks
+// K6 (dense contractions) — bf16 GEMM on the Hopper tensor cores: C[M,N] = act(A[M,K] · B[N,K]^T + bias)
+// with fp32 accumulation in registers.  Used for the linear layers of the policy/value networks
 // (a13: benchmark/torch/a2c/atari_model.py:46-49 fc 5184->512 and the heads; forward x·W^T).
 //
-// sm_100a structure (one 128 x BN output tile per CTA, BK = 64 bf16 = one 128-byte swizzle atom):
-//   warp 0   : TMA producer — cp.async.bulk.tensor 2-D tiles of A and B (SWIZZLE_128B) into a
-//              4..8-stage shared-memory ring, completion on per-stage "full" mbarriers
-//   warp 1   : allocates TMEM, issues tcgen05.mma (cta_group::1, kind::f16, M=128, N=BN, K=16) from
-//              ONE elected thread, 4 per stage; tcgen05.commit releases the stage ("empty") and,
-//              after the last k-block, signals "tmem_full"
-//   warps 2-5: epilogue — tcgen05.ld the 128 x BN fp32 accumulator (each warp its own 32-lane
-//              quarter), bias + optional ReLU, convert, store
+// sm_90a structure (one 128 x BN output tile per CTA, BK = 64 bf16 = one 128-byte swizzle atom):
+//   warp 0        : TMA producer — cp.async.bulk.tensor 2-D tiles of A and B (SWIZZLE_128B) into a
+//                   4..8-stage shared-memory ring, completion on per-stage "full" mbarriers
+//   warpgroups 1-2: consumers — warpgroup c issues wgmma.mma_async m64nBNk16 for rows [64c, 64c + 64) of the tile
+//                   (4 per stage, one stage kept in flight), releases each stage on its "empty" mbarrier once the
+//                   MMAs that read it have retired, then runs the epilogue (bias + optional ReLU / ReLU-backward
+//                   mask, convert, store) straight from its accumulator registers
 // Tensor-pipe bound: 2*M*N*K flops; operand traffic (M*K + N*K)*2 B + M*N*out B.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
 #include "tma.cuh"
+#include "wgmma.cuh"
 
 namespace rl {
 
@@ -23,98 +23,7 @@ constexpr int kGemmBK = 64;          // bf16 elements per k-block = 128 bytes
 // ring depth by tile width: the loop is bound by the L2/HBM latency of the TMA loads (bytes in flight per SM), so the
 // ring takes what shared memory allows — 8 stages up to BN = 64, 6 at BN = 128, 4 at BN = 256 (~200 KB)
 __host__ __device__ constexpr int gemm_stages(int bn) { return bn <= 64 ? 8 : (bn <= 128 ? 6 : 4); }
-constexpr int kGemmThreads = 192;    // 6 warps
-
-__device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorMap* map, int c0, int c1, void* mbar) {
-  tma_load_2d(smem_dst, map, c0, c1, mbar);
-}
-
-// ---- tcgen05 wrappers --------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrive once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(void* mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(mbar))
-               : "memory");
-}
-// ---- thread-block cluster helpers (2 x 2 multicast form) ---------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-// 2-D tile load delivered to the same shared-memory offset (and mbarrier) of every CTA in cta_mask
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* map, int c0, int c1, void* mbar,
-                                                      uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], "
-      "[%4], %5;\n" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(mbar)), "h"(cta_mask)
-      : "memory");
-}
-// arrive on the mbarrier at this offset in every CTA of cta_mask once this thread's MMAs have completed
-__device__ __forceinline__ void umma_commit_multicast(void* mbar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(
-                   smem_u32(mbar)),
-               "h"(cta_mask)
-               : "memory");
-}
-
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread (thread = lane/row)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// K-major operand tile in shared memory, 128-byte rows, SWIZZLE_128B (cute::UMMA::SmemDescriptor):
-//   start_address[0,14) = addr>>4 ; LBO[16,30) = 1 (unused for swizzled K-major) ; SBO[32,46) = 1024>>4
-//   version[46,48) = 1 (Blackwell) ; layout_type[61,64) = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// cute::UMMA::InstrDescriptor for kind::f16, BF16 x BF16 -> F32, both operands K-major
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+constexpr int kGemmThreads = 384;    // producer warpgroup (one active thread) + 2 consumer warpgroups
 
 struct GemmArgs {
   const float* bias;   // [N] or NULL
@@ -129,27 +38,21 @@ struct GemmArgs {
   int kb_per_split, ldp, mpad;
 };
 
-// CL (2 x 2 thread-block cluster, TMA multicast): the four CTAs of a cluster own a 256 x 2BN block of C.  The two CTAs
-// of one m-block need the same A tile, the two of one n-block the same B tile: each CTA loads HALF of its A tile
-// (map_a then has 64-row boxes) and half of its B tile and multicasts them to its partner, so every operand byte is
-// read from L2 once per cluster instead of once per CTA — the single-CTA form is L2-bandwidth bound at these shapes
-// (340 MB of operand re-reads for 4096 x 512 x 5184).  A stage of CTA X is written by X and its two partners, so X's
-// issuer releases it with ONE multicast tcgen05.commit to the three of them (empty barrier count 3).
-template <int BN, bool CL = false>
+__device__ __forceinline__ bool bf16_positive(__nv_bfloat16 h) { return __bfloat162float(h) > 0.f; }
+
+template <int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                       const __grid_constant__ CUtensorMap map_b,
                                                                       const GemmArgs g) {
   constexpr int A_STAGE = kGemmBM * kGemmBK * 2;     // 16 KB
   constexpr int B_STAGE = BN * kGemmBK * 2;
-  constexpr int TMEM_COLS = BN < 32 ? 32 : BN;
   constexpr int kGemmStages = gemm_stages(BN);
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   // SWIZZLE_128B atoms need 1024-byte alignment: align by hand (the launch reserves the slack)
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   unsigned char* sA = smem;                                     // [stages][128 rows][128 B]
   unsigned char* sB = smem + kGemmStages * A_STAGE;             // [stages][BN rows][128 B]
-  __shared__ __align__(8) unsigned long long full_bar[kGemmStages], empty_bar[kGemmStages], tmem_full_bar;
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) unsigned long long full_bar[kGemmStages], empty_bar[kGemmStages];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * kGemmBM, n0 = blockIdx.y * BN;
@@ -157,145 +60,91 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_bf16_tn_kernel(const __g
   const int kb0 = g.partial ? (int)blockIdx.z * g.kb_per_split : 0;
   const int num_kb = g.partial ? min(g.kb_per_split, num_kb_all - kb0) : num_kb_all;     // this CTA's k-blocks
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
     for (int s = 0; s < kGemmStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], CL ? 3 : 1);
+      mbar_init(&empty_bar[s], 2);          // one arrival per consumer warpgroup
     }
-    mbar_init(&tmem_full_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(&tmem_base_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  // cluster rank = x + 2 y: x = position along M (blockIdx.x & 1), y = along N; partners: rank ^ 2 shares this
-  // CTA's m-block (A tile), rank ^ 1 its n-block (B tile)
-  const uint32_t crank = CL ? cluster_ctarank() : 0u;
-  const uint16_t mask_a = (uint16_t)((1u << crank) | (1u << (crank ^ 2u)));
-  const uint16_t mask_b = (uint16_t)((1u << crank) | (1u << (crank ^ 1u)));
-  if (CL) cluster_sync_all();          // every CTA's barriers exist before a partner's TMA or commit can reach them
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   pdl_wait();            // chain kernel (launch_chain): A comes from the previous kernel of the stream
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===== TMA producer =====
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       for (int kb = 0; kb < num_kb; ++kb) {
         const int s = kb % kGemmStages;
         const uint32_t ph = (kb / kGemmStages) & 1;
         mbar_wait(&empty_bar[s], ph ^ 1u);                                  // slot free (first pass: immediately)
         mbar_arrive_expect_tx(&full_bar[s], A_STAGE + B_STAGE);
-        if (CL) {
-          const int ha = (int)(crank >> 1), hb = (int)(crank & 1u);        // which half of the shared tile this CTA fetches
-          tma_load_2d_multicast(sA + s * A_STAGE + ha * (A_STAGE / 2), &map_a, (kb0 + kb) * kGemmBK, m0 + ha * (kGemmBM / 2),
-                                &full_bar[s], mask_a);
-          tma_load_2d_multicast(sB + s * B_STAGE + hb * (B_STAGE / 2), &map_b, (kb0 + kb) * kGemmBK, n0 + hb * (BN / 2),
-                                &full_bar[s], mask_b);
-        } else {
-          tma_load_2d(sA + s * A_STAGE, &map_a, (kb0 + kb) * kGemmBK, m0, &full_bar[s]);
-          tma_load_2d(sB + s * B_STAGE, &map_b, (kb0 + kb) * kGemmBK, n0, &full_bar[s]);
-        }
+        tma_load_2d(sA + s * A_STAGE, &map_a, (kb0 + kb) * kGemmBK, m0, &full_bar[s]);
+        tma_load_2d(sB + s * B_STAGE, &map_b, (kb0 + kb) * kGemmBK, n0, &full_bar[s]);
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one thread) =====
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(kGemmBM, BN);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kGemmStages;
-        const uint32_t ph = (kb / kGemmStages) & 1;
-        mbar_wait(&full_bar[s], ph);                                        // TMA bytes have landed
-        tc_fence_after();
-        const uint64_t da = make_desc_sw128(smem_u32(sA + s * A_STAGE));
-        const uint64_t db = make_desc_sw128(smem_u32(sB + s * B_STAGE));
+    return;
+  }
+  // ===== consumers: warpgroup c owns rows [64c, 64c + 64) of the tile =====
+  const int c = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127;
+  float d[BN / 2];
 #pragma unroll
-        for (int k = 0; k < kGemmBK / 16; ++k) {
-          // advance 16 bf16 = 32 bytes along K inside the swizzle atom: +2 in the (addr >> 4) field
-          umma_bf16(tmem_base, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        if (CL)
-          umma_commit_multicast(&empty_bar[s], (uint16_t)(mask_a | mask_b));  // ... in this CTA and in both partners
-        else
-          umma_commit(&empty_bar[s]);                                       // frees the smem stage when the MMAs retire
-      }
-      umma_commit(&tmem_full_bar);                                          // accumulator complete
+  for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+  const uint32_t a_lo0 = gmma_lo(sA) + (uint32_t)(c * 64 * 128 >> 4), b_lo0 = gmma_lo(sB);
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % kGemmStages;
+    mbar_wait(&full_bar[s], (kb / kGemmStages) & 1);                      // TMA bytes have landed
+    wgmma_fence();
+    const uint32_t a_lo = a_lo0 + (uint32_t)(s * (A_STAGE >> 4)), b_lo = b_lo0 + (uint32_t)(s * (B_STAGE >> 4));
+#pragma unroll
+    for (int k = 0; k < kGemmBK / 16; ++k)      // 16 bf16 = 32 bytes along K inside the swizzle atom: +2 units
+      wgmma_bf16<BN>(d, gmma_desc(kGmmaHiSw128, a_lo + 2 * k), gmma_desc(kGmmaHiSw128, b_lo + 2 * k), (kb | k) != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();                                                      // k-block kb-1 has retired: free its stage
+    if (kb > 0 && t == 0) mbar_arrive(&empty_bar[(kb - 1) % kGemmStages]);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(d);
+  const int rbase = m0 + 64 * c;
+  if (g.partial) {
+    // raw accumulator dump (padded tile grid: no bounds), finished by gemm_splitk_reduce_kernel
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int row = rbase + gmma_row(t, i), col = n0 + gmma_col(t, i);
+      *reinterpret_cast<float2*>(g.partial + ((size_t)blockIdx.z * g.mpad + row) * g.ldp + col) = make_float2(d[i], d[i + 1]);
     }
-  } else {
-    // ===== epilogue: warps 2..5, TMEM lane quarter = warp % 4 =====
-    const int q = warp & 3;
-    mbar_wait(&tmem_full_bar, 0);
-    tc_fence_after();
-    const int row = m0 + q * 32 + lane;
-    const uint32_t tlane = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 16) {
-      float v[16];
-      tmem_ld16(tlane + (uint32_t)c0, v);
-      if (g.partial) {
-        // raw accumulator dump (padded tile grid: no bounds), finished by gemm_splitk_reduce_kernel
-        float* dst = g.partial + ((size_t)blockIdx.z * g.mpad + row) * g.ldp + n0 + c0;
+    return;
+  }
 #pragma unroll
-        for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(dst + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-        continue;
+  for (int i = 0; i < BN / 2; i += 2) {
+    const int row = rbase + gmma_row(t, i), col = n0 + gmma_col(t, i);
+    if (row >= g.M || col >= g.N) continue;
+    const bool two = col + 1 < g.N;
+    float v0 = d[i] + (g.bias ? g.bias[col] : 0.f), v1 = d[i + 1] + ((g.bias && two) ? g.bias[col + 1] : 0.f);
+    if (g.relu) v0 = fmaxf(v0, 0.f), v1 = fmaxf(v1, 0.f);
+    if (g.mask) {
+      const __nv_bfloat16* mrow = g.mask + (size_t)row * g.ldm + col;
+      if (!bf16_positive(mrow[0])) v0 = 0.f;
+      if (two && !bf16_positive(mrow[1])) v1 = 0.f;
+    }
+    if (g.out_f32) {
+      float* dst = reinterpret_cast<float*>(g.C) + (size_t)row * g.ldc + col;
+      if (two && (g.ldc & 1) == 0) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+      else {
+        dst[0] = v0;
+        if (two) dst[1] = v1;
       }
-      if (row < g.M) {
-        const int col = n0 + c0;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          float x = v[i] + ((g.bias && col + i < g.N) ? g.bias[col + i] : 0.f);
-          v[i] = g.relu ? fmaxf(x, 0.f) : x;
-        }
-        if (g.mask) {
-          const __nv_bfloat16* mrow = g.mask + (size_t)row * g.ldm + col;
-          if (col + 16 <= g.N && (g.ldm & 7) == 0 && (reinterpret_cast<uintptr_t>(g.mask) & 15u) == 0) {
-            // two 16-byte loads; keep where the saved activation is > 0 (bf16: sign clear and magnitude non-zero)
-            const uint4 m0 = __ldg(reinterpret_cast<const uint4*>(mrow)), m1 = __ldg(reinterpret_cast<const uint4*>(mrow) + 1);
-            const uint32_t mw[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              if ((mw[i] & 0x7fffu) == 0u || (mw[i] & 0x8000u)) v[2 * i] = 0.f;
-              if ((mw[i] & 0x7fff0000u) == 0u || (mw[i] & 0x80000000u)) v[2 * i + 1] = 0.f;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (col + i < g.N && !(__bfloat162float(mrow[i]) > 0.f)) v[i] = 0.f;
-          }
-        }
-        if (g.out_f32) {
-          float* dst = reinterpret_cast<float*>(g.C) + (size_t)row * g.ldc + col;
-          if (col + 16 <= g.N && (g.ldc & 3) == 0) {
-#pragma unroll
-            for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(dst + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-          } else {
-            for (int i = 0; i < 16 && col + i < g.N; ++i) dst[i] = v[i];
-          }
-        } else {
-          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(g.C) + (size_t)row * g.ldc + col;
-          if (col + 16 <= g.N && (g.ldc & 7) == 0) {
-            uint32_t pk[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * i], v[2 * i + 1]);
-              pk[i] = *reinterpret_cast<uint32_t*>(&h);
-            }
-            *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            *reinterpret_cast<uint4*>(dst + 8) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-          } else {
-            for (int i = 0; i < 16 && col + i < g.N; ++i) dst[i] = __float2bfloat16(v[i]);
-          }
-        }
+    } else {
+      __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(g.C) + (size_t)row * g.ldc + col;
+      if (two && (g.ldc & 1) == 0) *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
+      else {
+        dst[0] = __float2bfloat16(v0);
+        if (two) dst[1] = __float2bfloat16(v1);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (CL) cluster_sync_all();          // no CTA leaves while a partner may still multicast into it or signal its barriers
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // C[row, col] = act(sum_z partial[z][row][col] + bias[col]) in split order (deterministic)
@@ -327,8 +176,8 @@ __global__ void __launch_bounds__(256) gemm_splitk_reduce_kernel(const float* __
 // layer): a warp owns one row.  H[row, :] = relu(sum_z partial[z][row][:] + bias) (split-K reduce; or, with
 // partial == NULL, H is read as written by the GEMM epilogue), rounded to bf16 and stored; then
 // out2[row, n] = b2[n] + sum_c bf16(H[row, c]) * W2[n, c] for the N2 <= 32 head rows — fp32, fixed order (16-column
-// lane partials, xor-shuffle tree), so the per-step chain has one launch instead of reduce + a tensor-core GEMM whose
-// 7-8 us are all prologue at N2 = 18.
+// lane partials, xor-shuffle tree), so the per-step chain has one launch instead of reduce + a tensor-core GEMM that
+// is all prologue at N2 = 18.
 struct HeadsArgs {
   const __nv_bfloat16* W2;   // [N2, N] bf16
   const float* b2;           // [N2] or NULL
@@ -402,8 +251,8 @@ __global__ void __launch_bounds__(256) fc_reduce_heads_kernel(const float* __res
 }
 
 // The head alone, when H already exists (after the GEMM epilogue or the plain split-K reduce): out2 = H . W2^T + b2 with
-// warp-level mma.sync.m16n8k16 (bf16 x bf16 -> f32).  N2 <= 24 columns are a sliver of a tcgen05 tile — the UMMA kernel
-// spends its 7-8 us on barrier setup, TMEM allocation and the TMA ring for 8 k-blocks — while here a 16-row tile is
+// warp-level mma.sync.m16n8k16 (bf16 x bf16 -> f32).  N2 <= 24 columns are a sliver of a wgmma tile — that kernel
+// would spend its time on barrier setup and the TMA ring for 8 k-blocks — while here a 16-row tile is
 // four warps, each reducing a quarter of K straight from global memory (fragments are 4-byte loads in the operands'
 // native row-major layouts), then one shared-memory pass adds the four partial tiles in a fixed order.
 __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
@@ -492,26 +341,6 @@ static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const GemmA
   return 0;
 }
 
-// 2 x 2 cluster form: the tile grid is rounded up to even counts (out-of-range tiles load zeros and store nothing)
-template <int BN>
-static int launch_gemm_cluster(const CUtensorMap& ma, const CUtensorMap& mb, const GemmArgs& g, cudaStream_t st) {
-  const size_t smem = (size_t)gemm_stages(BN) * (kGemmBM * kGemmBK * 2 + BN * kGemmBK * 2) + 1024;
-  auto kern = gemm_bf16_tn_kernel<BN, true>;
-  RL_SMEM_OPTIN(kern);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(((g.M + kGemmBM - 1) / kGemmBM + 1) & ~1), (unsigned)(((g.N + BN - 1) / BN + 1) & ~1), 1);
-  cfg.blockDim = dim3(kGemmThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2, attr[0].val.clusterDim.y = 2, attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = pdl_enabled();
-  cfg.attrs = attr, cfg.numAttrs = 2;
-  return cudaLaunchKernelEx(&cfg, kern, ma, mb, g) == cudaSuccess ? 0 : -1;
-}
-
 }  // namespace rl
 
 using namespace rl;
@@ -520,13 +349,12 @@ static int gemm_launch(const void* A, const void* B, const float* bias, void* C,
                        int ldc, int relu, int out_f32, const void* mask, int ldm, void* workspace, size_t workspace_bytes,
                        rl_stream_t stream, const HeadsArgs* heads = nullptr);
 
-// 1 (default): 2 x 2 cluster + TMA multicast form for outputs of at least 2 x 2 tiles of width >= 128; 0: never.
-static int g_gemm_cluster = 1;
-static int g_heads_mma = 1;      // 1: mma.sync head kernel after the plain reduce; 0: warp-per-row CUDA-core kernel(s)
+// The 2 x 2 cluster + TMA multicast form of the B200 build is not part of the sm_90a kernels; 0 is the only setting.
 extern "C" int rl_debug_set_gemm_cluster(int enable) {
-  g_gemm_cluster = enable ? 1 : 0;
+  RL_CHECK_ARG(enable == 0, "gemm cluster form: not built for sm_90a (only 0 is accepted)");
   return RL_OK;
 }
+static int g_heads_mma = 1;      // 1: mma.sync head kernel after the plain reduce; 0: warp-per-row CUDA-core kernel(s)
 
 extern "C" int rl_gemm_bf16_tn(const void* A, const void* B, const float* bias, void* C, int M, int N, int K, int lda,
                                int ldb, int ldc, int relu, int out_f32, rl_stream_t stream) {
@@ -564,6 +392,13 @@ extern "C" int rl_gemm_bf16_tn_masked(const void* A, const void* B, void* C, con
   return gemm_launch(A, B, nullptr, C, M, N, K, lda, ldb, ldc, 0, out_f32, mask, ldm, nullptr, 0, stream);
 }
 
+static int device_sms() {
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return effective_sms(sms);
+}
+
 static int launch_heads(const float* partial, int splits, int mpad, int ldp, const float* bias, void* H, int ldh, int M,
                         int N, int relu, const HeadsArgs& hd, cudaStream_t st) {
   if (!partial && g_heads_mma && hd.N2 <= 8 * kHeadsMmaNT && N % 64 == 0 && ldh % 2 == 0)
@@ -573,7 +408,7 @@ static int launch_heads(const float* partial, int splits, int mpad, int ldp, con
                : -1;
   const size_t smem = (size_t)hd.N2 * N * 2;
   int blocks = (M + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   return launch_chain(fc_reduce_heads_kernel, dim3((unsigned)blocks), dim3(256), smem, st, partial, splits, mpad, ldp, bias,
                       (__nv_bfloat16*)H, ldh, M, N, relu, hd) == cudaSuccess
              ? 0
@@ -588,13 +423,11 @@ static int gemm_launch(const void* A, const void* B, const float* bias, void* C,
   RL_CHECK_ARG(lda >= K && ldb >= K && ldc >= N && (lda % 8) == 0 && (ldb % 8) == 0,
                "gemm_bf16_tn: lda/ldb must be >= K and multiples of 8 elements (TMA row pitch)");
   int BN = N > 128 ? 256 : (N > 64 ? 128 : (N > 32 ? 64 : 32));
-  // small problems: prefer narrower tiles until the grid covers about two thirds of the 148 SMs — but no further:
-  // one thread issues every tcgen05.mma at ~50 cycles each, so an N = 64 tile (32 tensor-core cycles per
-  // instruction) is issue-bound while N = 128 is not.  Measured for 4096 x 512 x 5184 (the actor's fc layer): BN 64
-  // = 256 CTAs 30.8 us, BN 128 = 128 CTAs 32.4 us, BN 256 = 64 CTAs 40.0 us — all L2-bandwidth bound (340 MB of
-  // operand re-reads per call); the fix is a 2-CTA cluster with TMA multicast, not the tile shape.
+  // small problems: prefer narrower tiles until the grid covers about two thirds of the SMs, but keep N >= 64 so
+  // that each wgmma instruction still carries enough tensor-core work per shared-memory operand read
+  const int sms = device_sms();
   const long long mt = (M + kGemmBM - 1) / kGemmBM;
-  while (BN > 64 && mt * ((N + BN - 1) / BN) < 100) BN >>= 1;
+  while (BN > 64 && mt * ((N + BN - 1) / BN) < (2 * sms) / 3) BN >>= 1;
   alignas(64) CUtensorMap ma, mb;
   if (make_tensor_map_bf16_sw128(&ma, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, kGemmBM) ||
       make_tensor_map_bf16_sw128(&mb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, (uint32_t)BN)) {
@@ -608,8 +441,8 @@ static int gemm_launch(const void* A, const void* B, const float* bias, void* C,
   // split-K: fewer output tiles than half the SMs and a long reduction (one CTA would walk >= 16 k-blocks alone)
   const int nt = (N + BN - 1) / BN, num_kb = (K + kGemmBK - 1) / kGemmBK;
   int splits = 1;
-  if (workspace && !mask && mt * nt * 2 <= 148 && num_kb >= 16) {
-    int want = (int)(148 / (mt * nt));
+  if (workspace && !mask && mt * nt * 2 <= sms && num_kb >= 16) {
+    int want = (int)(sms / (mt * nt));
     if (want > num_kb / 8) want = num_kb / 8;
     if (want > 8) want = 8;
     const int per = (num_kb + want - 1) / want;
@@ -621,25 +454,6 @@ static int gemm_launch(const void* A, const void* B, const float* bias, void* C,
     }
   }
   cudaStream_t st = (cudaStream_t)stream;
-  if (g_gemm_cluster && splits == 1 && BN >= 128 && mt >= 2 && nt >= 2) {
-    // 2 x 2 cluster: half-tile boxes, each half multicast to the partner CTA
-    if (make_tensor_map_bf16_sw128(&ma, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, kGemmBM / 2) ||
-        make_tensor_map_bf16_sw128(&mb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, (uint32_t)BN / 2)) {
-      set_error("gemm_bf16_tn: cuTensorMapEncodeTiled failed");
-      return RL_ERR_CUDA;
-    }
-    const int rc = BN == 256 ? launch_gemm_cluster<256>(ma, mb, g, st) : launch_gemm_cluster<128>(ma, mb, g, st);
-    if (rc) {
-      set_error("gemm_bf16_tn: cluster launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-      return RL_ERR_CUDA;
-    }
-    RL_CHECK_LAUNCH("rl_gemm_bf16_tn");
-    if (heads && launch_heads(nullptr, 0, 0, 0, nullptr, C, ldc, M, N, 0, *heads, st)) {
-      set_error("gemm_bf16_tn_heads: heads launch failed");
-      return RL_ERR_CUDA;
-    }
-    return RL_OK;
-  }
   switch (BN) {
     case 256: launch_gemm<256>(ma, mb, g, splits, st); break;
     case 128: launch_gemm<128>(ma, mb, g, splits, st); break;

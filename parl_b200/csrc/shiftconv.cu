@@ -1,9 +1,9 @@
-// K6 (convolutions, TMA-window form) — stride-1 NHWC bf16 convolution forward on tcgen05 where the A operand
-// is never gathered: a stride-1 conv over the row-major flattened pixel sequence is a sum of SHIFTED GEMMs
+// K6 (convolutions, TMA-window form) — stride-1 NHWC bf16 convolution forward on the Hopper tensor cores where the
+// A operand is never gathered: a stride-1 conv over the row-major flattened pixel sequence is a sum of SHIFTED GEMMs
 //     out[q, :] = bias + sum_{r,s} in[q + r*W + s, :] . W[(r,s)]^T        q = n*H*W + y*W + x
 // (positions with y >= Hout or x >= Wout are computed and dropped).  Per 128-position tile ONE 2-D TMA load
 // brings the input window rows [q0, q0 + 128 + (KH-1)*W + (KW-1)) into shared memory (SWIZZLE_128B); every
-// filter tap then issues tcgen05.mma with an smem descriptor that simply starts (r*W+s) rows further down
+// filter tap then issues wgmma with an smem descriptor that simply starts (r*W+s) rows further down
 // (the swizzle phase follows from the absolute shared-memory address).  Each input byte crosses L2->SM once per tile
 // instead of once per tap.  Stride-2/4 layers are brought to this form by space-to-depth of their INPUT
 // (conv1: rl_obs_stack_gather out_dtype 3; conv2: conv1's epilogue writes the padded 2x2-block layout).
@@ -12,77 +12,22 @@
 //   conv1  8x8/4/p1, 4->32   == 2x2/1 on [21,21,64]   -> [20,20,32] written as s2d2-padded [12,12,128]
 //   conv2  4x4/2/p2, 32->64  == 2x2/1 on [12,12,128]  -> [11,11,64]
 //   conv3  3x3/1,    64->64  == 3x3/1 on [11,11,64]   -> [9,9,64]
-// Roles: warp 0 TMA producer (window ring), warps 1 and 10 MMA issuers taking alternate tiles (weights
-// resident in smem, FOUR TMEM accumulators in flight; one issuing thread needs ~50 cycles per tcgen05.mma of
-// 16-64 tensor-core cycles, so a single issuer was the bound — ncu round 1), warps 2-9 epilogue in TWO groups of four warps that take alternate tiles (bias,
-// ReLU, bf16, layout-aware row store) — one group's tcgen05.ld -> convert -> store latency chain hides behind
-// the other's, which is what bounds these small-N tiles (16..72 MMAs of 128xNx16 per tile).
+// Roles: warp 0 TMA producer (window ring); consumer warpgroups 1 and 2 take alternate tiles of the CTA (weights
+// resident in smem): each issues the tile's wgmma m64nCOUT chains for both 64-row halves into two register
+// accumulators, frees the window slot once they retire, and runs the epilogue (bias, ReLU or ReLU-backward mask,
+// bf16, layout-aware store) from its registers — one warpgroup's epilogue overlaps the other's MMAs.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
 #include "tma.cuh"
 #include "u8win.cuh"
+#include "wgmma.cuh"
 
 namespace rl {
 
-__device__ __forceinline__ void s_tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void s_tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void s_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void s_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void s_umma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void s_commit(void* mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(mbar))
-               : "memory");
-}
-__device__ __forceinline__ void s_tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void s_mbar_arrive(void* mbar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(mbar)) : "memory");
-}
-// K-major SWIZZLE_128B operand starting at an arbitrary 128-byte row of a 1024-byte aligned swizzled buffer.
-// The hardware derives the swizzle phase from the absolute address, so base_offset (bits 49-51) stays 0
-// (measured on B200: setting it double-counts the phase, max error 4.3 vs 0.016).  Everything but the 14-bit
-// start-address field (address >> 4; shared memory is < 256 KB so the field never overflows) is constant, so the
-// issuing thread only ADDS 16-byte units to the low word: tap shift, k step (32 B) and weight block.
-constexpr uint32_t kDescHiSw128 = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);   // SBO, version 1, SWIZZLE_128B
-constexpr uint32_t kDescLoLbo1 = 1u << 16;                                            // LBO field = 1
-__device__ __forceinline__ uint64_t s_desc_from_lo(uint32_t lo) {                     // lo = (addr >> 4) + kDescLoLbo1
-  return ((uint64_t)kDescHiSw128 << 32) | (uint64_t)lo;
-}
-__host__ __device__ constexpr uint32_t s_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
 constexpr int kScBM = 128;
 constexpr int kScMaxStages = 8;      // window ring depth is chosen at launch from the shared memory left by the weights
-constexpr int kScEpiGroups = 2;      // epilogue warp groups (4 warps each) working on alternate tiles
-constexpr int kScAcc = 4;            // TMEM accumulators in flight (kScAcc * COUT <= 512 columns)
-constexpr int kScIssuer2 = 2 + 4 * kScEpiGroups;   // warp index of the second MMA issuer (odd tiles)
-constexpr int kScThreads = 32 * (kScIssuer2 + 1);
+constexpr int kScThreads = 384;      // producer warpgroup (warp 0 active) + 2 consumer warpgroups
 
 struct ShiftConvArgs {
   const float* bias;
@@ -115,33 +60,26 @@ __device__ __forceinline__ uint32_t s_pack_relu_bf16x2(float lo, float hi) {
 }
 
 // MODE 0: forward  (out = act(acc + bias), ReLU optional)     MODE 1: data gradient (out = acc * (mask > 0), mask optional)
-// The epilogue is the instruction-issue hot spot of these kernels (ncu round 1: ~85 % of the issue slots of the
-// data-gradient kernel), so it is kept to: tcgen05.ld, 4 LDS.128 of bias + 16 FADD or one HSET2 mask per pair,
-// one cvt(.relu).bf16x2 per pair, two 16-byte stores — no per-element branches.
 // U8IN (conv1 on the uint8 observation): map_in is the uint8 [Q][64] matrix, the producer fills a dense staging
-// ring and four more warps (11-14) convert each window into the bf16 SWIZZLE_128B ring (u8win.cuh).
+// ring and 256 more threads convert each window into the bf16 SWIZZLE_128B ring (u8win.cuh).
 template <int COUT, int CBLK, int KS, int MODE, bool U8IN = false>
 __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1)
     shiftconv_fwd_kernel(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_w,
                          const ShiftConvArgs g) {
   static_assert(!U8IN || CBLK == 1, "the uint8 window is one 64-channel block");
   constexpr int W_KB = COUT * 128;                        // one 64-wide weight k-block
-  constexpr int TMEM_COLS = kScAcc * COUT;                // 128 / 256 / 512: powers of two
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   constexpr int num_kb = KS * KS * CBLK;                  // square KS x KS filter
   const int win_bytes = (g.wrows * 128 + 1023) & ~1023;   // one 64-channel column block of the window
   unsigned char* sW = smem;                               // [num_kb][COUT][128 B]
   unsigned char* sWin = smem + ((num_kb * W_KB + 1023) & ~1023);   // [stages][CBLK][wrows][128 B]
-  __shared__ __align__(8) unsigned long long full_bar[kScMaxStages], empty_bar[kScMaxStages], w_bar, tmem_full[kScAcc], tmem_empty[kScAcc];
+  __shared__ __align__(8) unsigned long long full_bar[kScMaxStages], empty_bar[kScMaxStages], w_bar;
   __shared__ __align__(8) unsigned long long u8_full[kU8Stages], u8_empty[kU8Stages];
   const uint32_t nstages = (uint32_t)g.stages;
   unsigned char* sStage = sWin + nstages * CBLK * win_bytes;       // U8IN: [kU8Stages][wrows][64 B]
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ __align__(16) float s_bias[COUT];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (MODE == 0 && threadIdx.x < COUT) s_bias[threadIdx.x] = g.bias[threadIdx.x];
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_in);
     tma_prefetch_desc(&map_w);
@@ -154,29 +92,21 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
       mbar_init(&u8_empty[s], kU8Threads);
     }
     mbar_init(&w_bar, 1);
-    for (int b = 0; b < kScAcc; ++b) {
-      mbar_init(&tmem_full[b], 1);
-      mbar_init(&tmem_empty[b], 128);
-    }
     fence_mbar_init();
   }
-  if (warp == 1) s_tmem_alloc(&tmem_base_smem, TMEM_COLS);
-  s_fence_before();
   __syncthreads();
-  s_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   // resident weights: requested BEFORE the dependency wait (they are written by the operand refresh, at least two
   // kernels back in the stream), so the load overlaps the tail of the previous kernel
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 128) {
     mbar_arrive_expect_tx(&w_bar, (uint32_t)(num_kb * W_KB));
     for (int kb = 0; kb < num_kb; ++kb) tma_load_2d(sW + kb * W_KB, &map_w, kb * 64, 0, &w_bar);
   }
   pdl_wait();            // chain kernel (launch_chain): the input activations come from the previous kernel
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===== TMA producer: one window (CBLK column blocks) per tile =====
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       uint32_t s = 0, par = 1;
       if (U8IN) {
         const int sbytes = u8_stage_bytes(g.wrows);
@@ -197,7 +127,9 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
         }
       }
     }
-  } else if (U8IN && warp > kScIssuer2) {
+    return;
+  }
+  if (U8IN && threadIdx.x >= kScThreads) {
     // ===== uint8 -> bf16 window converters =====
     const int ct = threadIdx.x - kScThreads;
     const int sbytes = u8_stage_bytes(g.wrows);
@@ -206,206 +138,140 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
       mbar_wait(&u8_full[ss], fpar);
       mbar_wait(&empty_bar[s], epar);              // the MMAs that read this window slot have completed
-      s_fence_after();
       u8_window_to_bf16_sw128(sStage + ss * sbytes, sWin + s * win_bytes, g.wrows, ct, g.in_scale, bias);
       fence_proxy_async_smem();                    // generic-proxy stores -> visible to the tensor core's async proxy
-      s_mbar_arrive(&full_bar[s]);
-      s_mbar_arrive(&u8_empty[ss]);
+      mbar_arrive(&full_bar[s]);
+      mbar_arrive(&u8_empty[ss]);
       if (++s == nstages) s = 0, epar ^= 1u;
       if (++ss == kU8Stages) ss = 0, fpar ^= 1u;
     }
-  } else if (warp == 1 || warp == kScIssuer2) {
-    // ===== resident weights + MMA issue (issuer 0: even tiles of this CTA, issuer 1: odd tiles) =====
-    if (lane == 0) {
-      const uint32_t issuer = warp == 1 ? 0u : 1u;
-      mbar_wait(&w_bar, 0);
-      constexpr uint32_t idesc = s_idesc_bf16(kScBM, COUT);
-      // the issue loop is ONE thread's instruction stream: keep it to "add, add, mma" — tap shifts are
-      // loop-invariant registers (16-byte units: 8 per window row), weight offsets are compile-time constants
-      uint32_t tap_off[KS * KS];
+    return;
+  }
+  // ===== consumers: warpgroup c takes tiles it = c, c + 2, ... of this CTA =====
+  const int c = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127;
+  mbar_wait(&w_bar, 0);
+  // tap shifts in 16-byte descriptor units (8 per 128-byte window row)
+  uint32_t tap_off[KS * KS];
 #pragma unroll
-      for (int r = 0; r < KS; ++r)
+  for (int r = 0; r < KS; ++r)
 #pragma unroll
-        for (int sx = 0; sx < KS; ++sx)
-          tap_off[r * KS + sx] = (uint32_t)(g.flip ? (KS - 1 - r) * g.W + (KS - 1 - sx) : r * g.W + sx) * 8u;
-      const uint32_t w_lo = (smem_u32(sW) >> 4) + kDescLoLbo1, win_lo0 = (smem_u32(sWin) >> 4) + kDescLoLbo1;
-      const uint32_t win16 = (uint32_t)win_bytes >> 4;
-      uint32_t s = issuer, buf = issuer, full_par = 0, empty_par = 1;        // nstages >= 2, kScAcc = 4
-      for (long long tile = blockIdx.x + (long long)issuer * gridDim.x; tile < g.num_tiles; tile += 2 * gridDim.x) {
-        mbar_wait(&tmem_empty[buf], empty_par);
-        mbar_wait(&full_bar[s], full_par);
-        s_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * COUT;
-        const uint32_t a_lo = win_lo0 + s * (CBLK * win16);
+    for (int sx = 0; sx < KS; ++sx)
+      tap_off[r * KS + sx] = (uint32_t)(g.flip ? (KS - 1 - r) * g.W + (KS - 1 - sx) : r * g.W + sx) * 8u;
+  const uint32_t w_lo = gmma_lo(sW), win_lo0 = gmma_lo(sWin);
+  const uint32_t win16 = (uint32_t)win_bytes >> 4;
+  float bias_r[MODE == 0 ? COUT / 2 : 1];           // bias of the column of each accumulator element
+  if (MODE == 0) {
 #pragma unroll
-        for (int tap = 0; tap < KS * KS; ++tap) {
+    for (int i = 0; i < COUT / 2; ++i) bias_r[i] = __ldg(g.bias + gmma_col(t, i));
+  }
+  const bool relu = g.relu != 0;
+  const bool has_mask = MODE == 1 && g.mask != nullptr;
+  const int HW = g.H * g.W;
+  uint32_t s = (uint32_t)c, full_par = 0;
+  for (long long tile = blockIdx.x + (long long)c * gridDim.x; tile < g.num_tiles; tile += 2 * gridDim.x) {
+    float d[2][COUT / 2];                            // rows [0, 64) and [64, 128) of the tile
+    mbar_wait(&full_bar[s], full_par);
+    wgmma_fence();
+    const uint32_t a_lo = win_lo0 + s * (CBLK * win16);
 #pragma unroll
-          for (int cb = 0; cb < CBLK; ++cb) {
+    for (int h = 0; h < 2; ++h) {
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              s_umma(d_tmem, s_desc_from_lo(a_lo + cb * win16 + tap_off[tap] + 2u * k),
-                     s_desc_from_lo(w_lo + (uint32_t)((tap * CBLK + cb) * (W_KB >> 4) + 2 * k)), idesc,
-                     (tap | cb | k) != 0 ? 1u : 0u);
+      for (int tap = 0; tap < KS * KS; ++tap) {
+#pragma unroll
+        for (int cb = 0; cb < CBLK; ++cb) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            wgmma_bf16<COUT>(d[h], gmma_desc(kGmmaHiSw128, a_lo + h * 512u + cb * win16 + tap_off[tap] + 2u * k),
+                             gmma_desc(kGmmaHiSw128, w_lo + (uint32_t)((tap * CBLK + cb) * (W_KB >> 4) + 2 * k)),
+                             (tap | cb | k) != 0 ? 1u : 0u);
+        }
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(d[0]);
+    wgmma_fence_regs(d[1]);
+    if (t == 0) mbar_arrive(&empty_bar[s]);        // the window slot is free for the next TMA load
+    s += 2;
+    if (s >= nstages) s -= nstages, full_par ^= 1u;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {               // the thread's two rows of this half: r0 and r0 + 8
+        const int q = (int)tile * kScBM + 64 * h + gmma_row(t, 2 * rr);
+        const int n = q / HW;
+        const int rem = q - n * HW;
+        const int y = rem / g.W, x = rem - y * g.W;
+        const bool valid = q < g.Q && y < g.Hout && x < g.Wout;
+        size_t obase = 0;
+        if (g.out_mode == 0) {
+          obase = ((size_t)(n * g.OGH + y) * g.OGW + x) * COUT;
+        } else if (g.out_mode == 1) {
+          // conv1 -> conv2 input: zero-padded by 2, 2x2 space-to-depth: [n, (y+2)/2, (x+2)/2, ((y&1)*2 + (x&1))*COUT + c]
+          const int yp = y + 2, xp = x + 2;
+          obase = (((size_t)n * 12 + (yp >> 1)) * 12 + (xp >> 1)) * (4 * COUT) + (size_t)(((yp & 1) * 2 + (xp & 1)) * COUT);
+        }
+#pragma unroll
+        for (int j = 0; j < COUT / 8; ++j) {
+          const int i = 4 * j + 2 * rr, col = gmma_col(t, i);
+          bool ok = valid;
+          size_t dst_off = obase + col;
+          if (g.out_mode == 2) {
+            // channel block (dy,dx) of position (Y,X) is pixel (2Y+dy-2, 2X+dx-2) of the 20x20 image, 32 channels
+            const int blk = col >> 5, py = 2 * y + (blk >> 1) - 2, px = 2 * x + (blk & 1) - 2;
+            ok = q < g.Q && py >= 0 && py < 20 && px >= 0 && px < 20;
+            dst_off = (((size_t)n * 21 + py) * 21 + px) * 32 + (col & 31);
           }
-        }
-        s_commit(&empty_bar[s]);
-        s_commit(&tmem_full[buf]);
-        s += 2;
-        if (s >= nstages) s -= nstages, full_par ^= 1u;
-        buf += 2;
-        if (buf >= kScAcc) buf -= kScAcc, empty_par ^= 1u;
-      }
-    }
-  } else {
-    // ===== epilogue (warps 2 .. 2 + 4 * kScEpiGroups - 1) =====
-    const int qd = warp & 3;                        // TMEM lane quarter this warp may read
-    const int grp = (warp - 2) >> 2;                // epilogue group: tiles it = grp, grp + 2, ...
-    const int HW = g.H * g.W;
-    // the bias lives in registers: a broadcast LDS per 4 channels per tile would cost shared-memory wavefronts on
-    // the pipe that already limits these kernels (tensor-core operand reads + TMEM reads, ncu round 2)
-    float bias_r[MODE == 0 ? COUT : 1];
-    if (MODE == 0) {
-#pragma unroll
-      for (int i = 0; i < COUT; ++i) bias_r[i] = s_bias[i];
-    }
-    for (uint32_t it = (uint32_t)grp; blockIdx.x + (long long)it * gridDim.x < g.num_tiles; it += kScEpiGroups) {
-      const int tile = blockIdx.x + (int)it * gridDim.x;
-      const uint32_t buf = it % kScAcc;
-      const int q = tile * kScBM + qd * 32 + lane;
-      // ReLU mask of this row (accumulator grid [Q, COUT]): issued BEFORE waiting for the accumulator so that the
-      // global-memory latency overlaps the MMAs of this tile
-      const bool has_mask = MODE == 1 && g.mask != nullptr;
-      uint4 mk[COUT / 8];
-      if (has_mask && q < g.Q) {
-        const uint4* mp = reinterpret_cast<const uint4*>(g.mask + (size_t)q * COUT);
-#pragma unroll
-        for (int i = 0; i < COUT / 8; ++i) mk[i] = __ldg(mp + i);
-      }
-      const int n = q / HW;
-      const int rem = q - n * HW;
-      const int y = rem / g.W, x = rem - y * g.W;
-      mbar_wait(&tmem_full[buf], (it / kScAcc) & 1u);
-      s_fence_after();
-      const bool valid = q < g.Q && y < g.Hout && x < g.Wout;
-      size_t obase = 0;
-      if (g.out_mode == 0) {
-        obase = ((size_t)(n * g.OGH + y) * g.OGW + x) * COUT;
-      } else if (g.out_mode == 1) {
-        // conv1 -> conv2 input: zero-padded by 2, 2x2 space-to-depth: [n, (y+2)/2, (x+2)/2, ((y&1)*2 + (x&1))*COUT + c]
-        const int yp = y + 2, xp = x + 2;
-        obase = (((size_t)n * 12 + (yp >> 1)) * 12 + (xp >> 1)) * (4 * COUT) + (size_t)(((yp & 1) * 2 + (xp & 1)) * COUT);
-      }
-      const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16) + buf * COUT;
-      const bool relu = g.relu != 0;
-#pragma unroll
-      for (int c0 = 0; c0 < COUT; c0 += 16) {
-        float v[16];
-        s_tmem_ld16(taddr + (uint32_t)c0, v);
-        bool ok = valid;
-        size_t dst_off = obase + c0;
-        if (g.out_mode == 2) {
-          // channel block (dy,dx) of position (Y,X) is pixel (2Y+dy-2, 2X+dx-2) of the 20x20 image, 32 channels
-          const int blk = c0 >> 5, py = 2 * y + (blk >> 1) - 2, px = 2 * x + (blk & 1) - 2;
-          ok = q < g.Q && py >= 0 && py < 20 && px >= 0 && px < 20;
-          dst_off = (((size_t)n * 21 + py) * 21 + px) * 32 + (c0 & 31);   // a lane writes 2 x 128 contiguous bytes
-        }
-        if (ok) {
-          uint32_t pk[8];
+          if (!ok) continue;
+          uint32_t pk;
           if (MODE == 0) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] += bias_r[c0 + i];
-            if (relu) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) pk[i] = s_pack_relu_bf16x2(v[2 * i], v[2 * i + 1]);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) pk[i] = s_pack_bf16x2(v[2 * i], v[2 * i + 1]);
-            }
+            const float v0 = d[h][i] + bias_r[i], v1 = d[h][i + 1] + bias_r[i + 1];
+            pk = relu ? s_pack_relu_bf16x2(v0, v1) : s_pack_bf16x2(v0, v1);
           } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) pk[i] = s_pack_bf16x2(v[2 * i], v[2 * i + 1]);
+            pk = s_pack_bf16x2(d[h][i], d[h][i + 1]);
             if (has_mask) {
-              // ReLU backward: keep the gradient where the saved activation is > 0 — one packed bf16x2 compare per pair
-              const uint4 mk0 = mk[c0 / 8], mk1 = mk[c0 / 8 + 1];
-              const uint32_t mw[8] = {mk0.x, mk0.y, mk0.z, mk0.w, mk1.x, mk1.y, mk1.z, mk1.w};
-              const __nv_bfloat162 zero2 = __floats2bfloat162_rn(0.f, 0.f);
-#pragma unroll
-              for (int i = 0; i < 8; ++i) pk[i] &= __hgt2_mask(*reinterpret_cast<const __nv_bfloat162*>(&mw[i]), zero2);
+              // ReLU backward: keep the gradient where the saved activation is > 0 — one packed bf16x2 compare
+              const uint32_t mw = __ldg(reinterpret_cast<const unsigned int*>(g.mask + (size_t)q * COUT + col));
+              pk &= __hgt2_mask(*reinterpret_cast<const __nv_bfloat162*>(&mw), __floats2bfloat162_rn(0.f, 0.f));
             }
           }
-          uint4* dst = reinterpret_cast<uint4*>(g.out + dst_off);
-          dst[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          dst[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+          *reinterpret_cast<uint32_t*>(g.out + dst_off) = pk;
         }
       }
-      s_fence_before();
-      s_mbar_arrive(&tmem_empty[buf]);
     }
   }
-  s_fence_before();
-  __syncthreads();
-  if (warp == 1) s_tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Column-tap-fused form (opt-in experiment, rl_debug_set_shiftconv_form(1)).  ncu on the form above
-// (profiles/r02_conv_forms.txt): these small-N layers run at ~1 shared-memory wavefront per clock per SM — the
-// shared-memory data pipe is the bound — of which two thirds are the tensor core's OPERAND reads (every tcgen05.mma
-// streams its 128-row A slice, 32 wavefronts of 128 B, for only N = 32..64 output columns, once per filter tap) and
-// one quarter the epilogue's TMEM reads (tcgen05.ld goes through the same pipe: 32 wavefronts per 32x32b.x16).
-// Here the KS taps of one filter ROW share one A read: the B tile of a (row r, channel block)
-// step stacks the weights of its KS column taps, N' = KS * COUT, so the accumulator row of window row p holds
-//     D[p, (s, co)] = sum_{r, ci} in[p + r*W, ci] * W[co, (r, s, ci)]
-// and the epilogue finishes out[p, co] = sum_s D[p + s, (s, co)]: the accumulator row of window row p + s sits in
-// TMEM lane p + s, i.e. in the NEIGHBOURING thread of the epilogue warp, so the shift is a warp shuffle; the last
-// KS-1 lanes of each warp get their neighbours' values from the next warp through a small shared-memory exchange
-// (one named barrier per tile and epilogue group), and a tile of 128 window rows yields 128-(KS-1) output rows.
-// MMAs per tile: KS*CBLK*4 instead of KS*KS*CBLK*4; A wavefronts divided by KS.
-// MEASURED (51 200 samples, B200): conv1 865 vs 686 us, conv2 758 vs 562, conv3 752 vs 416 — slower: the operand
-// wavefronts do drop (conv1 113 M -> 68 M, tensor pipe busy 85 % -> 43 %) but the accumulator is KS times wider, so
-// the TMEM reads grow by what the operand reads shrink (conv1: 45 M -> 80 M LSU-pipe wavefronts) and the epilogue's
-// instruction chain (shuffles, exchange, barrier) becomes the critical path.  Bit-exact on the integer tests.
+// Column-tap form (rl_debug_set_shiftconv_form(1)): an independent cross-check of the tap / shift bookkeeping of the
+// form above.  The KS taps of a filter COLUMN s share no window shift: the tile computes, per column tap s,
+//     D_s[p, co] = sum_{r, ci} in[p + r*W, ci] * W[co, (r, s, ci)]
+// and the epilogue finishes out[p, co] = sum_s D_s[p + shift(s), co] (shift(s) = s, or KS-1-s for the transposed
+// conv), so the column shift is applied to the OUTPUT rows through a shared-memory accumulator instead of to the
+// operand descriptor.  A tile of 128 window rows yields 128 - (KS-1) output rows.  Both consumer warpgroups work on
+// the same tile (rows [64c, 64c + 64)); the column taps are accumulated in shift order 0, 1, .. into the fp32 tile,
+// one 256-thread barrier per phase.
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void s_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-template <int COUT, int KS>
-struct SfShape {
-  static constexpr int NP = KS * COUT;                          // accumulator columns (s, co)
-  static constexpr int NACC = (512 / NP) >= 4 ? 4 : 2;          // accumulators in flight
-  static constexpr int ST = kScBM - (KS - 1);                   // output rows per 128-row tile
-  static constexpr int XCH = 4 * (KS - 1) * (KS - 1) * COUT;    // [warp][shift-1][lane][co] floats handed to the previous warp
-  static constexpr int PART = 4 * (KS - 1) * COUT;              // [warp][boundary lane][co] partial sums
-  static constexpr int XCH_FLOATS = XCH + PART;                 // one exchange buffer
-  static constexpr int XCH_BYTES = kScEpiGroups * 2 * XCH_FLOATS * 4;
-};
-
 template <int COUT, int CBLK, int KS, int MODE, bool U8IN = false>
 __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1)
-    shiftconv_sfused_kernel(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_w,
+    shiftconv_coltap_kernel(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_w,
                             const ShiftConvArgs g) {
   static_assert(!U8IN || CBLK == 1, "the uint8 window is one 64-channel block");
-  using SH = SfShape<COUT, KS>;
-  constexpr int NP = SH::NP, NACC = SH::NACC, ST = SH::ST;
-  constexpr int W_KB = COUT * 128;                        // one (tap, 64-channel block) weight tile
-  constexpr int TMEM_COLS = NACC * NP <= 128 ? 128 : (NACC * NP <= 256 ? 256 : 512);
+  constexpr int W_KB = COUT * 128;
+  constexpr int ST = kScBM - (KS - 1);                    // output rows per tile
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   constexpr int num_kb = KS * KS * CBLK;
   const int win_bytes = (g.wrows * 128 + 1023) & ~1023;
-  unsigned char* sW = smem;                               // [r][cb][s][COUT][128 B]
+  unsigned char* sW = smem;                               // [tap = r*KS + s][CBLK][COUT][128 B]
   unsigned char* sWin = smem + ((num_kb * W_KB + 1023) & ~1023);
-  __shared__ __align__(8) unsigned long long full_bar[kScMaxStages], empty_bar[kScMaxStages], w_bar, tmem_full[kScAcc], tmem_empty[kScAcc];
+  __shared__ __align__(8) unsigned long long full_bar[kScMaxStages], empty_bar[kScMaxStages], w_bar;
   __shared__ __align__(8) unsigned long long u8_full[kU8Stages], u8_empty[kU8Stages];
   const uint32_t nstages = (uint32_t)g.stages;
-  unsigned char* sStage = sWin + nstages * CBLK * win_bytes;                       // U8IN: [kU8Stages][wrows][64 B]
-  float* sXch = reinterpret_cast<float*>(sStage + (U8IN ? kU8Stages * u8_stage_bytes(g.wrows) : 0));
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ __align__(16) float s_bias[COUT];
+  unsigned char* sStage = sWin + nstages * CBLK * win_bytes;
+  float* sAcc = reinterpret_cast<float*>(sStage + (U8IN ? kU8Stages * u8_stage_bytes(g.wrows) : 0));   // [128][COUT]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (MODE == 0 && threadIdx.x < COUT) s_bias[threadIdx.x] = g.bias[threadIdx.x];
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_in);
     tma_prefetch_desc(&map_w);
@@ -418,21 +284,19 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
       mbar_init(&u8_empty[s], kU8Threads);
     }
     mbar_init(&w_bar, 1);
-    for (int b = 0; b < kScAcc; ++b) {
-      mbar_init(&tmem_full[b], 1);
-      mbar_init(&tmem_empty[b], 128);
-    }
     fence_mbar_init();
   }
-  if (warp == 1) s_tmem_alloc(&tmem_base_smem, TMEM_COLS);
-  s_fence_before();
   __syncthreads();
-  s_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
+  if (threadIdx.x == 128) {
+    mbar_arrive_expect_tx(&w_bar, (uint32_t)(num_kb * W_KB));
+    for (int kb = 0; kb < num_kb; ++kb) tma_load_2d(sW + kb * W_KB, &map_w, kb * 64, 0, &w_bar);
+  }
+  pdl_wait();
+  pdl_trigger();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===== TMA producer: one window per tile; tiles advance by ST rows =====
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       uint32_t s = 0, par = 1;
       if (U8IN) {
         const int sbytes = u8_stage_bytes(g.wrows);
@@ -453,208 +317,116 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
         }
       }
     }
-  } else if (U8IN && warp > kScIssuer2) {
-    // ===== uint8 -> bf16 window converters =====
+    return;
+  }
+  if (U8IN && threadIdx.x >= kScThreads) {
     const int ct = threadIdx.x - kScThreads;
     const int sbytes = u8_stage_bytes(g.wrows);
     const float bias = -8388608.0f * g.in_scale;
     uint32_t s = 0, epar = 1, ss = 0, fpar = 0;
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
       mbar_wait(&u8_full[ss], fpar);
-      mbar_wait(&empty_bar[s], epar);              // the MMAs that read this window slot have completed
-      s_fence_after();
+      mbar_wait(&empty_bar[s], epar);
       u8_window_to_bf16_sw128(sStage + ss * sbytes, sWin + s * win_bytes, g.wrows, ct, g.in_scale, bias);
-      fence_proxy_async_smem();                    // generic-proxy stores -> visible to the tensor core's async proxy
-      s_mbar_arrive(&full_bar[s]);
-      s_mbar_arrive(&u8_empty[ss]);
+      fence_proxy_async_smem();
+      mbar_arrive(&full_bar[s]);
+      mbar_arrive(&u8_empty[ss]);
       if (++s == nstages) s = 0, epar ^= 1u;
       if (++ss == kU8Stages) ss = 0, fpar ^= 1u;
     }
-  } else if (warp == 1 || warp == kScIssuer2) {
-    // ===== resident weights + MMA issue (issuer 0: even tiles of this CTA, issuer 1: odd tiles) =====
-    if (lane == 0) {
-      const uint32_t issuer = warp == 1 ? 0u : 1u;
-      if (issuer == 0) {
-        mbar_arrive_expect_tx(&w_bar, (uint32_t)(num_kb * W_KB));
-        // slot ((r * CBLK + cb) * KS + s) <- columns of tap (r, s), channel block cb of the [Cout, (r,s,ci)] matrix
-        for (int r = 0; r < KS; ++r)
-          for (int cb = 0; cb < CBLK; ++cb)
-            for (int sx = 0; sx < KS; ++sx)
-              tma_load_2d(sW + ((r * CBLK + cb) * KS + sx) * W_KB, &map_w, ((r * KS + sx) * CBLK + cb) * 64, 0, &w_bar);
-      }
-      mbar_wait(&w_bar, 0);
-      constexpr uint32_t idesc = s_idesc_bf16(kScBM, NP);
-      uint32_t row_off[KS];                            // window-row shift of filter row r, 16-byte units
+    return;
+  }
+  // ===== consumers: warpgroup c owns rows [64c, 64c + 64) of every tile of this CTA =====
+  const int c = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127;
+  mbar_wait(&w_bar, 0);
+  uint32_t row_off[KS];                                   // window shift of filter row r, 16-byte units
 #pragma unroll
-      for (int r = 0; r < KS; ++r) row_off[r] = (uint32_t)((g.flip ? KS - 1 - r : r) * g.W) * 8u;
-      const uint32_t w_lo = (smem_u32(sW) >> 4) + kDescLoLbo1, win_lo0 = (smem_u32(sWin) >> 4) + kDescLoLbo1;
-      const uint32_t win16 = (uint32_t)win_bytes >> 4;
-      uint32_t s = issuer, buf = issuer % NACC, full_par = 0, empty_par = 1;
-      for (long long tile = blockIdx.x + (long long)issuer * gridDim.x; tile < g.num_tiles; tile += 2 * gridDim.x) {
-        mbar_wait(&tmem_empty[buf], empty_par);
-        mbar_wait(&full_bar[s], full_par);
-        s_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * NP;
-        const uint32_t a_lo = win_lo0 + s * (CBLK * win16);
+  for (int r = 0; r < KS; ++r) row_off[r] = (uint32_t)((g.flip ? KS - 1 - r : r) * g.W) * 8u;
+  const uint32_t w_lo = gmma_lo(sW), win_lo0 = gmma_lo(sWin);
+  const uint32_t win16 = (uint32_t)win_bytes >> 4;
+  float bias_r[MODE == 0 ? COUT / 2 : 1];
+  if (MODE == 0) {
 #pragma unroll
-        for (int r = 0; r < KS; ++r) {
+    for (int i = 0; i < COUT / 2; ++i) bias_r[i] = __ldg(g.bias + gmma_col(t, i));
+  }
+  const bool relu = g.relu != 0;
+  const bool has_mask = MODE == 1 && g.mask != nullptr;
+  const int HW = g.H * g.W;
+  uint32_t s = 0, full_par = 0;
+  for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
+    mbar_wait(&full_bar[s], full_par);
+    const uint32_t a_lo = win_lo0 + s * (CBLK * win16) + (uint32_t)c * 512u;
 #pragma unroll
-          for (int cb = 0; cb < CBLK; ++cb) {
+    for (int sh = 0; sh < KS; ++sh) {
+      const int sc = g.flip ? KS - 1 - sh : sh;          // the column tap whose output shift is sh
+      float d[COUT / 2];
+      wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              s_umma(d_tmem, s_desc_from_lo(a_lo + cb * win16 + row_off[r] + 2u * k),
-                     s_desc_from_lo(w_lo + (uint32_t)((r * CBLK + cb) * KS * (W_KB >> 4) + 2 * k)), idesc,
-                     (r | cb | k) != 0 ? 1u : 0u);
-          }
+      for (int r = 0; r < KS; ++r)
+#pragma unroll
+        for (int cb = 0; cb < CBLK; ++cb)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            wgmma_bf16<COUT>(d, gmma_desc(kGmmaHiSw128, a_lo + cb * win16 + row_off[r] + 2u * k),
+                             gmma_desc(kGmmaHiSw128, w_lo + (uint32_t)(((r * KS + sc) * CBLK + cb) * (W_KB >> 4) + 2 * k)),
+                             (r | cb | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      // both warpgroups: the previous phase's accumulation (or the previous tile's epilogue) is complete
+      named_bar_sync(1, 256);
+      if (sh == KS - 1 && threadIdx.x == 128) mbar_arrive(&empty_bar[s]);   // every MMA of this window has retired
+#pragma unroll
+      for (int i = 0; i < COUT / 2; i += 2) {
+        const int p = 64 * c + gmma_row(t, i) - sh;       // output row this accumulator row contributes to
+        if (p < 0) continue;
+        float2* cell = reinterpret_cast<float2*>(sAcc + p * COUT + gmma_col(t, i));
+        if (sh == 0) {
+          *cell = make_float2(d[i], d[i + 1]);
+        } else {
+          const float2 o = *cell;
+          *cell = make_float2(o.x + d[i], o.y + d[i + 1]);
         }
-        s_commit(&empty_bar[s]);
-        s_commit(&tmem_full[buf]);
-        s += 2;
-        if (s >= nstages) s -= nstages, full_par ^= 1u;
-        buf += 2;
-        if (buf >= (uint32_t)NACC) buf -= NACC, empty_par ^= 1u;
       }
     }
-  } else {
-    // ===== epilogue (warps 2 .. 2 + 4 * kScEpiGroups - 1) =====
-    const int qd = warp & 3;                        // TMEM lane quarter this warp may read
-    const int grp = (warp - 2) >> 2;                // epilogue group: tiles it = grp, grp + 2, ...
-    const int HW = g.H * g.W;
-    constexpr int BL0 = 32 - (KS - 1);              // first lane whose column taps reach into the next warp
-    const bool bnd = lane >= BL0;
-    const bool has_mask = MODE == 1 && g.mask != nullptr;
-    const bool relu = g.relu != 0;
-    for (uint32_t it = (uint32_t)grp; blockIdx.x + (long long)it * gridDim.x < g.num_tiles; it += kScEpiGroups) {
-      const int tile = blockIdx.x + (int)it * gridDim.x;
-      const uint32_t buf = it % NACC;
-      const int row = qd * 32 + lane;
-      const int q = tile * ST + row;
-      const bool inrange = row < ST && q < g.Q;
-      uint4 mk[COUT / 8];
-      if (has_mask && inrange) {
-        const uint4* mp = reinterpret_cast<const uint4*>(g.mask + (size_t)q * COUT);
+    if (++s == nstages) s = 0, full_par ^= 1u;
+    named_bar_sync(1, 256);
 #pragma unroll
-        for (int i = 0; i < COUT / 8; ++i) mk[i] = __ldg(mp + i);
-      }
+    for (int i = 0; i < COUT / 2; i += 2) {
+      const int p = 64 * c + gmma_row(t, i), col = gmma_col(t, i);
+      const int q = tile * ST + p;
+      if (p >= ST || q >= g.Q) continue;
+      const float2 v = *reinterpret_cast<const float2*>(sAcc + p * COUT + col);
       const int n = q / HW;
       const int rem = q - n * HW;
       const int y = rem / g.W, x = rem - y * g.W;
-      const bool valid = inrange && y < g.Hout && x < g.Wout;
-      size_t obase = 0;
+      bool ok = y < g.Hout && x < g.Wout;
+      size_t dst_off;
       if (g.out_mode == 0) {
-        obase = ((size_t)(n * g.OGH + y) * g.OGW + x) * COUT;
+        dst_off = ((size_t)(n * g.OGH + y) * g.OGW + x) * COUT + col;
       } else if (g.out_mode == 1) {
         const int yp = y + 2, xp = x + 2;
-        obase = (((size_t)n * 12 + (yp >> 1)) * 12 + (xp >> 1)) * (4 * COUT) + (size_t)(((yp & 1) * 2 + (xp & 1)) * COUT);
+        dst_off = (((size_t)n * 12 + (yp >> 1)) * 12 + (xp >> 1)) * (4 * COUT) + (size_t)(((yp & 1) * 2 + (xp & 1)) * COUT) + col;
+      } else {
+        const int blk = col >> 5, py = 2 * y + (blk >> 1) - 2, px = 2 * x + (blk & 1) - 2;
+        ok = py >= 0 && py < 20 && px >= 0 && px < 20;
+        dst_off = (((size_t)n * 21 + py) * 21 + px) * 32 + (col & 31);
       }
-      // bias / activation / mask, bf16 pack and the layout-aware store of 16 channels of this thread's output row
-      auto emit = [&](int c0, float (&v)[16]) {
-        bool ok = valid;
-        size_t dst_off = obase + c0;
-        if (g.out_mode == 2) {
-          const int blk = c0 >> 5, py = 2 * y + (blk >> 1) - 2, px = 2 * x + (blk & 1) - 2;
-          ok = inrange && py >= 0 && py < 20 && px >= 0 && px < 20;
-          dst_off = (((size_t)n * 21 + py) * 21 + px) * 32 + (c0 & 31);
-        }
-        if (!ok) return;
-        uint32_t pk[8];
-        if (MODE == 0) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 b4 = *reinterpret_cast<const float4*>(&s_bias[c0 + 4 * i]);
-            v[4 * i] += b4.x, v[4 * i + 1] += b4.y, v[4 * i + 2] += b4.z, v[4 * i + 3] += b4.w;
-          }
-          if (relu) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) pk[i] = s_pack_relu_bf16x2(v[2 * i], v[2 * i + 1]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) pk[i] = s_pack_bf16x2(v[2 * i], v[2 * i + 1]);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) pk[i] = s_pack_bf16x2(v[2 * i], v[2 * i + 1]);
-          if (has_mask) {
-            const __nv_bfloat162 zero2 = __floats2bfloat162_rn(0.f, 0.f);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const uint4 m4 = mk[c0 / 8 + (i >> 2)];
-              const uint32_t mw = (i & 3) == 0 ? m4.x : ((i & 3) == 1 ? m4.y : ((i & 3) == 2 ? m4.z : m4.w));
-              pk[i] &= __hgt2_mask(*reinterpret_cast<const __nv_bfloat162*>(&mw), zero2);
-            }
-          }
-        }
-        uint4* dst = reinterpret_cast<uint4*>(g.out + dst_off);
-        dst[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        dst[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-      };
-      float* xb = sXch + (grp * 2 + (int)((it >> 1) & 1u)) * SH::XCH_FLOATS;     // exchange buffer of this tile
-      float* part = xb + SH::XCH;
-      mbar_wait(&tmem_full[buf], (it / NACC) & 1u);
-      s_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16) + buf * NP;
-#pragma unroll
-      for (int c0 = 0; c0 < COUT; c0 += 16) {
-        float v[16];
-        // the column tap whose window shift is 0: s = 0 (forward) or KS-1 (transposed)
-        s_tmem_ld16(taddr + (uint32_t)((g.flip ? KS - 1 : 0) * COUT + c0), v);
-#pragma unroll
-        for (int sh = 1; sh < KS; ++sh) {
-          float u[16];
-          s_tmem_ld16(taddr + (uint32_t)((g.flip ? KS - 1 - sh : sh) * COUT + c0), u);
-          if (qd > 0 && lane < sh) {                 // rows the previous warp's last lanes need
-            float4* d = reinterpret_cast<float4*>(xb + ((qd * (KS - 1) + (sh - 1)) * (KS - 1) + lane) * COUT + c0);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) d[i] = make_float4(u[4 * i], u[4 * i + 1], u[4 * i + 2], u[4 * i + 3]);
-          }
-          const bool have = lane + sh < 32;
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float t = __shfl_down_sync(0xffffffffu, u[i], sh);
-            v[i] += have ? t : 0.f;
-          }
-        }
-        if (!bnd) {
-          emit(c0, v);
-        } else {
-          float4* d = reinterpret_cast<float4*>(part + (qd * (KS - 1) + (lane - BL0)) * COUT + c0);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) d[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+      if (!ok) continue;
+      uint32_t pk;
+      if (MODE == 0) {
+        const float v0 = v.x + bias_r[i], v1 = v.y + bias_r[i + 1];
+        pk = relu ? s_pack_relu_bf16x2(v0, v1) : s_pack_bf16x2(v0, v1);
+      } else {
+        pk = s_pack_bf16x2(v.x, v.y);
+        if (has_mask) {
+          const uint32_t mw = __ldg(reinterpret_cast<const unsigned int*>(g.mask + (size_t)q * COUT + col));
+          pk &= __hgt2_mask(*reinterpret_cast<const __nv_bfloat162*>(&mw), __floats2bfloat162_rn(0.f, 0.f));
         }
       }
-      s_fence_before();
-      s_mbar_arrive(&tmem_empty[buf]);               // the accumulator is free: the rest works from shared memory
-      s_bar_sync(1 + grp, 128);
-      if (bnd && qd < 3) {                           // qd == 3: rows >= ST, no output
-#pragma unroll
-        for (int c0 = 0; c0 < COUT; c0 += 16) {
-          float v[16];
-          const float4* pp = reinterpret_cast<const float4*>(part + (qd * (KS - 1) + (lane - BL0)) * COUT + c0);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float4 t = pp[i];
-            v[4 * i] = t.x, v[4 * i + 1] = t.y, v[4 * i + 2] = t.z, v[4 * i + 3] = t.w;
-          }
-#pragma unroll
-          for (int sh = 1; sh < KS; ++sh) {
-            if (lane + sh >= 32) {
-              const float4* xp = reinterpret_cast<const float4*>(
-                  xb + (((qd + 1) * (KS - 1) + (sh - 1)) * (KS - 1) + (lane + sh - 32)) * COUT + c0);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float4 t = xp[i];
-                v[4 * i] += t.x, v[4 * i + 1] += t.y, v[4 * i + 2] += t.z, v[4 * i + 3] += t.w;
-              }
-            }
-          }
-          emit(c0, v);
-        }
-      }
+      *reinterpret_cast<uint32_t*>(g.out + dst_off) = pk;
     }
   }
-  s_fence_before();
-  __syncthreads();
-  if (warp == 1) s_tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 static int sc_make_map(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint32_t box_rows) {
@@ -694,37 +466,35 @@ static void launch_shiftconv(const CUtensorMap& mi, const CUtensorMap& mw, const
 }
 
 template <int COUT, int CBLK, int KS, int MODE, bool U8IN = false>
-static void launch_sfused(const CUtensorMap& mi, const CUtensorMap& mw, const ShiftConvArgs& g, int num_kb, int sms,
+static void launch_coltap(const CUtensorMap& mi, const CUtensorMap& mw, const ShiftConvArgs& g, int num_kb, int sms,
                           cudaStream_t st) {
   const size_t win = (size_t)((g.wrows * 128 + 1023) & ~1023);
   const size_t smem = (size_t)((num_kb * COUT * 128 + 1023) & ~1023) + (size_t)g.stages * CBLK * win + 1024 +
-                      (U8IN ? u8_ring_bytes(g.wrows) : 0) + SfShape<COUT, KS>::XCH_BYTES;
-  auto kern = shiftconv_sfused_kernel<COUT, CBLK, KS, MODE, U8IN>;
+                      (U8IN ? u8_ring_bytes(g.wrows) : 0) + (size_t)kScBM * COUT * sizeof(float);
+  auto kern = shiftconv_coltap_kernel<COUT, CBLK, KS, MODE, U8IN>;
   RL_SMEM_OPTIN(kern);
   const int grid = g.num_tiles < sms ? g.num_tiles : sms;
-  kern<<<grid, U8IN ? kScThreads + kU8Threads : kScThreads, smem, st>>>(mi, mw, g);
+  launch_chain(kern, dim3(grid), dim3(U8IN ? kScThreads + kU8Threads : kScThreads), smem, st, mi, mw, g);
 }
 
 }  // namespace rl
 
 using namespace rl;
 
-// 0 (default): one tcgen05.mma group per filter tap (shiftconv_fwd_kernel); 1: column-tap-fused form
-// (shiftconv_sfused_kernel) — measured SLOWER on B200 (see its header), kept as the documented experiment and as
-// an independent cross-check of the tap/shift bookkeeping.
+// Tile form of the window conv.  0 (default): one MMA chain per filter tap, the shift applied to the operand window
+// (shiftconv_fwd_kernel); 1: per filter column, the column shift applied to the output rows (shiftconv_coltap_kernel),
+// an independent cross-check of the tap / shift bookkeeping.
 static int g_sc_form = 0;
 extern "C" int rl_debug_set_shiftconv_form(int form) {
-  RL_CHECK_ARG(form == 0 || form == 1, "shiftconv form must be 0 (per-tap) or 1 (column taps fused)");
+  RL_CHECK_ARG(form == 0 || form == 1, "shiftconv form must be 0 (per-tap) or 1 (column taps)");
   g_sc_form = form;
   return RL_OK;
 }
 
-// Former triage hook.  Measured on B200 (round 1): the tensor core swizzles on ABSOLUTE shared-memory address
-// bits, so a descriptor that starts at an arbitrary 128-byte row of a 1024-byte aligned swizzled buffer needs NO
-// base_offset (setting it double-counted the phase: max error 4.3 vs 0.016).  The field is now hard-wired to 0
-// in the issue loop; asking for 1 is an error.
+// The descriptor base_offset field stays 0: the swizzle phase follows from the absolute shared-memory address of the
+// shifted window row, so setting it would count the phase twice.  Asking for 1 is an error.
 extern "C" int rl_debug_set_shiftconv_base_offset(int enable) {
-  RL_CHECK_ARG(enable == 0, "shiftconv base_offset=1 was measured wrong on B200 and has been removed");
+  RL_CHECK_ARG(enable == 0, "shiftconv base_offset must be 0 (the swizzle phase comes from the shared-memory address)");
   return RL_OK;
 }
 
@@ -743,9 +513,9 @@ static int shiftconv_launch(const void* in, const void* weight, const float* bia
   g.Hout = Hout, g.Wout = Wout, g.OGH = OGH, g.OGW = OGW;
   const long long Q = (long long)N * H * W;
   RL_CHECK_ARG(Q < (1LL << 31), "%s: too many positions", name);
-  const int fused = g_sc_form && KW * Cout <= 256;                    // N' = KW * Cout accumulator columns per tile
-  const int tile_rows = fused ? kScBM - (KW - 1) : kScBM;             // output rows per 128-row tile
-  g.Q = (int)Q, g.wrows = kScBM + (KH - 1) * W + (fused ? 0 : KW - 1), g.relu = relu, g.out_mode = out_mode;
+  const int coltap = g_sc_form == 1;
+  const int tile_rows = coltap ? kScBM - (KW - 1) : kScBM;            // output rows per 128-row tile
+  g.Q = (int)Q, g.wrows = kScBM + (KH - 1) * W + (coltap ? 0 : KW - 1), g.relu = relu, g.out_mode = out_mode;
   g.row_shift = transposed ? -((KH - 1) * W + (KW - 1)) : 0, g.flip = transposed;
   g.mask = (const __nv_bfloat16*)mask, g.in_scale = in_scale;
   RL_CHECK_ARG(g.wrows <= 256, "%s: window of %d rows exceeds the TMA box limit", name, g.wrows);
@@ -753,9 +523,8 @@ static int shiftconv_launch(const void* in, const void* weight, const float* bia
   const int cblk = Cin / 64, num_kb = KH * KW * cblk;
   const size_t win = (size_t)((g.wrows * 128 + 1023) & ~1023);
   {
-    // exchange buffers of the fused epilogue: 2 groups x 2 buffers x 4 warps x (KW-1) lanes x KW x Cout floats
-    const size_t xch = fused ? (size_t)2 * 2 * 4 * (KW - 1) * KW * Cout * 4 : 0;
-    const size_t budget = 220 * 1024 - ((size_t)num_kb * Cout * 128 + 2048) - (u8in ? u8_ring_bytes(g.wrows) : 0) - xch;
+    const size_t acc = coltap ? (size_t)kScBM * Cout * sizeof(float) : 0;    // column-tap form: fp32 output tile
+    const size_t budget = 220 * 1024 - ((size_t)num_kb * Cout * 128 + 2048) - (u8in ? u8_ring_bytes(g.wrows) : 0) - acc;
     long long st = (long long)(budget / ((size_t)cblk * win));
     if (st > kScMaxStages) st = kScMaxStages;
     // the dgrad epilogue reads the ReLU mask through L1: leave the unified L1/shared array some cache
@@ -770,24 +539,25 @@ static int shiftconv_launch(const void* in, const void* weight, const float* bia
     set_error("%s: cuTensorMapEncodeTiled failed", name);
     return RL_ERR_CUDA;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   sms = effective_sms(sms);
   cudaStream_t st = (cudaStream_t)stream;
   // instantiations: the layers of the Atari actor-critic and their data gradients (2x2 and 3x3 filters)
   const int key = (u8in ? 1000000 : 0) + (transposed ? 100000 : 0) + Cout * 100 + cblk * 10 + KH;
-  if (fused) {
+  if (coltap) {
     switch (key) {
-      case 1003212: launch_sfused<32, 1, 2, 0, true>(mi, mw, g, num_kb, sms, st); break;  // conv1 fwd, uint8 input
-      case 3212: launch_sfused<32, 1, 2, 0>(mi, mw, g, num_kb, sms, st); break;          // conv1 fwd
-      case 6422: launch_sfused<64, 2, 2, 0>(mi, mw, g, num_kb, sms, st); break;          // conv2 fwd
-      case 6413: launch_sfused<64, 1, 3, 0>(mi, mw, g, num_kb, sms, st); break;          // conv3 fwd
-      case 6412: launch_sfused<64, 1, 2, 0>(mi, mw, g, num_kb, sms, st); break;
-      case 6423: launch_sfused<64, 2, 3, 0>(mi, mw, g, num_kb, sms, st); break;
-      case 106413: launch_sfused<64, 1, 3, 1>(mi, mw, g, num_kb, sms, st); break;        // conv3 dgrad
-      case 112812: launch_sfused<128, 1, 2, 1>(mi, mw, g, num_kb, sms, st); break;       // conv2 dgrad
-      case 106412: launch_sfused<64, 1, 2, 1>(mi, mw, g, num_kb, sms, st); break;
+      case 1003212: launch_coltap<32, 1, 2, 0, true>(mi, mw, g, num_kb, sms, st); break;
+      case 3212: launch_coltap<32, 1, 2, 0>(mi, mw, g, num_kb, sms, st); break;
+      case 6422: launch_coltap<64, 2, 2, 0>(mi, mw, g, num_kb, sms, st); break;
+      case 6413: launch_coltap<64, 1, 3, 0>(mi, mw, g, num_kb, sms, st); break;
+      case 6412: launch_coltap<64, 1, 2, 0>(mi, mw, g, num_kb, sms, st); break;
+      case 6423: launch_coltap<64, 2, 3, 0>(mi, mw, g, num_kb, sms, st); break;
+      case 106413: launch_coltap<64, 1, 3, 1>(mi, mw, g, num_kb, sms, st); break;
+      case 112812: launch_coltap<128, 1, 2, 1>(mi, mw, g, num_kb, sms, st); break;
+      case 106412: launch_coltap<64, 1, 2, 1>(mi, mw, g, num_kb, sms, st); break;
+      case 112813: launch_coltap<128, 1, 3, 1>(mi, mw, g, num_kb, sms, st); break;
       default:
         set_error("%s: no instantiation for Cout=%d Cin=%d %dx%d", name, Cout, Cin, KH, KW);
         return RL_ERR_BAD_ARG;

@@ -1,4 +1,4 @@
-// TMA (cp.async.bulk.tensor) + mbarrier helpers for sm_100a, and host-side tensor-map creation
+// TMA (cp.async.bulk.tensor) + mbarrier helpers for sm_90a, and host-side tensor-map creation
 // through the driver entry point (no link-time libcuda dependency).
 #pragma once
 #include <cuda.h>
@@ -16,6 +16,9 @@ __device__ __forceinline__ void mbar_init(void* mbar, uint32_t count) {
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
+__device__ __forceinline__ void mbar_arrive(void* mbar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(mbar)) : "memory");
+}
 __device__ __forceinline__ void mbar_arrive_expect_tx(void* mbar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(smem_u32(mbar)), "r"(bytes) : "memory");
 }

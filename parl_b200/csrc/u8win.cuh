@@ -6,7 +6,7 @@
 // converter threads (4 per row, 16 input bytes each) write the 128-byte bf16 rows of the operand window exactly
 // where a SWIZZLE_128B tensor-map load would have put them — 16-byte chunk j of row r lands at chunk j ^ (r & 7)
 // (the window base is 1024-byte aligned) — then fence.proxy.async + mbarrier.arrive hand the window to the
-// tcgen05 issuers.  byte -> bf16(byte * scale) uses the same 2^23 magic-number FMA and cvt.rn.bf16x2 as the
+// wgmma consumers.  byte -> bf16(byte * scale) uses the same 2^23 magic-number FMA and cvt.rn.bf16x2 as the
 // bf16 gather (rl_obs_stack_gather out_dtype 3), so both input forms give bit-identical operands.
 #pragma once
 #include <cuda.h>
@@ -22,22 +22,15 @@ constexpr int kU8Threads = 256;    // converter threads (8 warps: two per schedu
 #ifdef __CUDACC__
 __device__ __forceinline__ int u8_stage_bytes(int wrows) { return (wrows * 64 + 1023) & ~1023; }
 
-// 16 bytes -> 16 x bf16(byte * scale): per byte one PRMT (2^23 magic number), half a packed FFMA2, half a cvt.bf16x2
+// 16 bytes -> 16 x bf16(byte * scale): per byte one PRMT (2^23 magic number), one FFMA, half a cvt.bf16x2
 __device__ __forceinline__ void u8x16_to_bf16(const uint4 in, float scale, float bias, uint32_t (&pk)[8]) {
   const uint32_t w[4] = {in.x, in.y, in.z, in.w};
-  unsigned long long sc2, bi2;
-  asm("mov.b64 %0, {%1, %1};\n" : "=l"(sc2) : "f"(scale));
-  asm("mov.b64 %0, {%1, %1};\n" : "=l"(bi2) : "f"(bias));
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    unsigned long long m01, m23, r01, r23;
-    asm("mov.b64 %0, {%1, %2};\n" : "=l"(m01) : "r"(__byte_perm(w[i], 0x4B000000u, 0x7540u)), "r"(__byte_perm(w[i], 0x4B000000u, 0x7541u)));
-    asm("mov.b64 %0, {%1, %2};\n" : "=l"(m23) : "r"(__byte_perm(w[i], 0x4B000000u, 0x7542u)), "r"(__byte_perm(w[i], 0x4B000000u, 0x7543u)));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;\n" : "=l"(r01) : "l"(m01), "l"(sc2), "l"(bi2));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;\n" : "=l"(r23) : "l"(m23), "l"(sc2), "l"(bi2));
-    float f0, f1, f2, f3;
-    asm("mov.b64 {%0, %1}, %2;\n" : "=f"(f0), "=f"(f1) : "l"(r01));
-    asm("mov.b64 {%0, %1}, %2;\n" : "=f"(f2), "=f"(f3) : "l"(r23));
+    const float f0 = __fmaf_rn(__uint_as_float(__byte_perm(w[i], 0x4B000000u, 0x7540u)), scale, bias);
+    const float f1 = __fmaf_rn(__uint_as_float(__byte_perm(w[i], 0x4B000000u, 0x7541u)), scale, bias);
+    const float f2 = __fmaf_rn(__uint_as_float(__byte_perm(w[i], 0x4B000000u, 0x7542u)), scale, bias);
+    const float f3 = __fmaf_rn(__uint_as_float(__byte_perm(w[i], 0x4B000000u, 0x7543u)), scale, bias);
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;\n" : "=r"(pk[2 * i]) : "f"(f1), "f"(f0));
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;\n" : "=r"(pk[2 * i + 1]) : "f"(f3), "f"(f2));
   }

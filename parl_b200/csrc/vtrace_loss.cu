@@ -166,10 +166,11 @@ __device__ __forceinline__ SoftmaxStats softmax_stats(const float* __restrict__ 
   const float l2S = lg2_approx(S);
   const float inv = __fdividef(1.0f, S);
   const float logSy = lg2_approx(Sy) * kLN2;
-  const float Hn = (W * inv - l2S) * kLN2;            // sum_j p_j log p_j
+  // explicit fma / rounding: every template instance must give the same bits (TMA and cp.async tile paths agree)
+  const float Hn = fmaf(W, inv, -l2S) * kLN2;          // sum_j p_j log p_j
   r.nm = nm, r.l2S = l2S, r.inv = inv;
   r.H = -Hn;
-  r.KL = Hn - Y * inv + my + logSy;                   // sum_j p_j (log p_j - log q_j)
+  r.KL = __fadd_rn(__fadd_rn(fmaf(-Y, inv, Hn), my), logSy);   // sum_j p_j (log p_j - log q_j)
   r.la = (fmaf(st[act], kL2E, nm) - l2S) * kLN2;
   r.lma = sb[act] - my - logSy;
   return r;
@@ -335,8 +336,9 @@ __global__ void __launch_bounds__(kNT, 7) vtrace_loss_kernel(const VtraceLossArg
         const float vs_n = __fadd_rn(acc_n, e_vn);                     // :128-129 (bootstrap at the end)
         const float adv = __fmul_rn(e_rpg, __fsub_rn(__fadd_rn(e_r, __fmul_rn(e_g, vs_n)), e_v));   // :136-137
         const float dv = e_v - vs;
-        sum_pi -= ss.la * adv;                                          // impala.py:67-68
-        sum_vf += 0.5f * dv * dv;                                       // :71-72
+        // explicit fma: the rounding must not depend on how the compiler contracts each template instance
+        sum_pi = fmaf(-ss.la, adv, sum_pi);                             // impala.py:67-68
+        sum_vf = fmaf(0.5f * dv, dv, sum_vf);                           // :71-72
         p.d_values[g] = p.vf_coeff * dv;
         if (p.vs_out) p.vs_out[t * B + b0 + bl_] = vs;
         if (p.pg_out) p.pg_out[t * B + b0 + bl_] = adv;
@@ -480,17 +482,16 @@ __global__ void __launch_bounds__(128) vtrace_returns_kernel(const float* __rest
 // ---------------------------------------------------------------------------
 // v8 (default for time-major TMA shapes with T <= 64, B % 4 == 0, even A <= 18): the K1 of the C3 learner batch.
 //
-// What bounded v4 at T=50, B=4096 (profiles/r02_k1_ncu.txt): 914 warp-instructions per 32 elements at 38 % issue
-// utilisation (three shared-memory sweeps with loop overhead, 3 block syncs per tile, a scan on warp 0 only) inside
-// ONE wave in which every CTA loads, then computes, then stores in lock-step — DRAM busy 20 %.  v8 keeps the CTA
-// shape "4 env columns x all T rows" (the scan never leaves the CTA, one wave of B/4 CTAs, 7 resident per SM) and
-// changes what happens inside it:
+// v4 spends three shared-memory sweeps with loop overhead, 3 block syncs per tile and a scan on warp 0 only per
+// element, and its CTAs load, then compute, then store in lock-step.  v8 keeps the CTA shape "4 env columns x all T
+// rows" (the scan never leaves the CTA; 7 CTAs resident per SM, so the B/4 = 1024 CTAs of B = 4096 are 1.1 waves on
+// the 132 SMs of an H100) and changes what happens inside it:
 //   * the tile is fetched as TWO half-tiles in time (later half first: it heads the backward recurrence), each with
 //     its own mbarrier; all four TMA loads are in flight from the first instruction, so the second half streams in
 //     while the first is being computed, and its gradient rows leave by TMA while the second half is computed;
 //   * 4 warps = one (t,b) element per thread per half; the element's 2A logits are read from shared memory ONCE
 //     into registers as 64-bit pairs (stride-18-word LDS.64: conflict-free), all arithmetic on packed pairs
-//     (fma/add/mul.f32x2), exponentials kept in registers for the gradient (no second MUFU pass, no re-read);
+//     (fma2/add2/mul2), exponentials kept in registers for the gradient (no second MUFU pass, no re-read);
 //   * the recurrence acc_t = delta_t + k_t acc_{t+1} is a 3-step shuffle suffix scan of affine maps inside each warp
 //     (8 rows), composed across the 4 warps after ONE block sync per half, carry between the halves in shared memory;
 //   * loss partials: one float4 per CTA, last CTA (ticket) reduces them in fixed order in fp64, overlapped with
@@ -505,26 +506,23 @@ __device__ __forceinline__ u64 pk2(float lo, float hi) {
 __device__ __forceinline__ void upk2(u64 v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
+// sm_90 has no packed f32x2 arithmetic: each pair op is two scalar round-to-nearest ops (same results)
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-  u64 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  upk2(a, a0, a1), upk2(b, b0, b1), upk2(c, c0, c1);
+  return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ u64 add2(u64 a, u64 b) {
-  u64 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1), upk2(b, b0, b1);
+  return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-  u64 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1), upk2(b, b0, b1);
+  return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
-__device__ __forceinline__ float max3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 // mbarrier wait with a hardware suspend-time hint (the warp sleeps instead of spinning on the LSU)
 __device__ __forceinline__ void mbar_wait_suspend(void* mbar, uint32_t parity) {
   asm volatile(
@@ -770,8 +768,8 @@ __global__ void __launch_bounds__(kV8Warps * 32, 7)     // 7 CTAs x 4 warps per 
   if (lane == 0) s_red[0][warp] = sum_pi, s_red[1][warp] = sum_vf, s_red[2][warp] = sum_ent, s_red[3][warp] = sum_kl;
   __syncthreads();
   // thread 0: gradient stores, the CTA's partial (one float4), the ticket.  The CTA that draws the last ticket reduces
-  // all partials (L2-resident) with EVERY load in flight at once: 8 independent float4 loads per thread — a loop of
-  // dependent L2 round trips here was 5 us of single-warp tail in the first v8 capture (profiles/r02_k1_v8_ncu.txt).
+  // all partials (L2-resident) with EVERY load in flight at once: 8 independent float4 loads per thread, so the
+  // single-CTA tail is one L2 round trip instead of a loop of dependent ones.
   if (tid == 0) {
     if (R0 > 0) tma_store_2d(&maps.dl[0], b0 * A_, 0, s_x + R1 * kRowBytes);
     else tma_store_2d(&maps.dl[1], b0 * A_, 0, s_x);

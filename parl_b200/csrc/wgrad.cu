@@ -1,412 +1,89 @@
 // K6 (convolution weight gradient, TMA-window form) — for a stride-1 NHWC conv written as shifted GEMMs
 //     out[q, co] = sum_t sum_ci in[q + off_t, ci] W_t[co, ci]
 // the weight gradient is a sum over ALL positions of outer products
-//     dW_t[co, ci] = sum_q dout_grid[q, co] * in[q + off_t, ci]
+//     dW_t[co, ci] = sum_q in[q + off_t, ci] * dout_grid[q, co]
 // i.e. per tap a GEMM whose reduction (K) dimension is the position index q.  Both operands are read exactly
-// as they lie in HBM — rows = positions, 128 contiguous bytes = 64 channels — through the same TMA windows as
-// the forward kernel and consumed by tcgen05.mma as MN-MAJOR operands (a_major = b_major = 1): A = dout tile
-// (M = 64 output channels), B = input window starting off_t rows down (N = 64 input channels), K = 16
-// positions per instruction.  Accumulators for all (tap, channel-block) pairs stay in TMEM across the CTA's
-// whole persistent loop over position tiles; taps are split over CTA groups when they exceed 512 columns.
-// Partials are dumped once per CTA and reduced in fixed order by a second kernel (deterministic).
-//
-// Issue rate.  With M = 64 tiles of K = 16 the tensor core needs only 16-32 cycles per instruction, so ONE
-// issuing thread (about 50 cycles per tcgen05.mma even with the descriptors reduced to "add to the low word")
-// was the bound (ncu round 1: tensor pipe 18-40 % active, issuer never waiting on data).  Two warps issue now,
-// each owning a disjoint half of the CTA's filter taps (= disjoint TMEM columns); both wait on the same "full"
-// barrier and both commit to the stage's "empty" barrier (count 2).
+// as they lie in HBM — rows = positions, contiguous channels — through the same TMA windows as the forward kernel and
+// consumed by wgmma as MN-MAJOR operands: A = input window starting off_t rows down (M = 64 input channels of one
+// channel block, SWIZZLE_128B), B = dout tile (N = Cout; SWIZZLE_128B for 64 channels, SWIZZLE_64B for 32), K = 16
+// positions per instruction.  Every (tap, channel block) pair is an accumulator "slot" of 64 x Cout fp32 registers
+// that stays in the registers of one consumer warpgroup across the CTA's whole persistent loop over position tiles.
+// The bias gradient rides along as one more slot whose A operand is a constant tile of ones,
+//     D_b[m, co] += sum_q 1 * dout[q, co]        (every row m holds the column sums; row 0 is read back)
+// so the gradient grid is not streamed from HBM a second time by a column-sum kernel.  Slots beyond what two
+// warpgroups hold (kWgSlots each) are split over CTA groups.  Partials are dumped once per CTA and reduced in fixed
+// order by a second kernel (deterministic).
 #include <cuda_bf16.h>
 
 #include "common.cuh"
 #include "tma.cuh"
 #include "u8win.cuh"
+#include "wgmma.cuh"
 
 namespace rl {
 
-__device__ __forceinline__ void w_tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void w_tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void w_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void w_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void w_umma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void w_commit(void* mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(mbar))
-               : "memory");
-}
-__device__ __forceinline__ void w_tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-// Shared-memory descriptors.  Only the 14-bit start-address field (address >> 4, shared memory < 256 KB) varies,
-// so the issuing threads keep "lo" words = (address >> 4) + kWgLoLbo1 and ADD 16-byte offsets to them.
-//   MN-major SWIZZLE_128B (cute canonical ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units): 64 MN-elements = one
-//     128-byte row per K index, 8 rows per 1024-byte swizzle atom (SBO = 1024 B between K-groups of 8); LBO unused.
-//   MN-major SWIZZLE_64B  (((4,n),(8,k)):((1,LBO),(4,SBO)), layout_type 4): 32 MN-elements = one 64-byte row per
-//     K index, 8 rows per 512-byte atom.
-__device__ __forceinline__ void w_mbar_arrive(void* mbar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(mbar)) : "memory");
-}
-constexpr uint32_t kWgLoLbo1 = 1u << 16;
-constexpr uint32_t kWgHiSw128 = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-constexpr uint32_t kWgHiSw64 = (uint32_t)(512 >> 4) | (1u << 14) | (4u << 29);
-__device__ __forceinline__ uint64_t w_desc(uint32_t hi, uint32_t lo) { return ((uint64_t)hi << 32) | (uint64_t)lo; }
-// kind::f16, BF16 x BF16 -> F32, A and B MN-major (bits 15, 16)
-__host__ __device__ constexpr uint32_t w_idesc_bf16_mn(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-
 constexpr int kWgBM = 128;            // positions (K of the GEMM) per tile
 constexpr int kWgMaxStages = 6;
-constexpr int kWgThreads = 224;       // warp 0 TMA, warps 1 and 6 MMA issuers (disjoint taps), warps 2-5 TMEM dump
-constexpr int kWgTapsPerIssuer = 5;   // <= 10 filter taps per CTA group
+constexpr int kWgThreads = 384;       // producer warpgroup (warp 0 active) + 2 consumer warpgroups
+constexpr int kWgSlots = 4;           // accumulator slots per consumer warpgroup (4 x 64 x 64 fp32 = 128 registers)
+constexpr int kWgMaxCtas = 160;       // grid bound the workspace is sized for
 
 struct WgradArgs {
-  float* partials;                    // [gridDim.x][128 lanes][ncols_max] raw TMEM dumps
-  int W, KH, KW;
-  int Q, wrows, num_tiles;
-  int ngroups, taps_per_group, ncols_max;
-  int stages;
-};
-
-template <int CBLK>
-__global__ void __launch_bounds__(kWgThreads, 1) wgrad_window_kernel(const __grid_constant__ CUtensorMap map_dout,
-                                                                     const __grid_constant__ CUtensorMap map_x,
-                                                                     const WgradArgs g) {
-  extern __shared__ __align__(1024) unsigned char smem_dyn[];
-  unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-  const int win_bytes = (g.wrows * 128 + 1023) & ~1023;
-  const int stage_bytes = kWgBM * 128 + CBLK * win_bytes;           // dout tile + input window blocks
-  __shared__ __align__(8) unsigned long long full_bar[kWgMaxStages], empty_bar[kWgMaxStages], done_bar;
-  const uint32_t nstages = (uint32_t)g.stages;
-  __shared__ uint32_t tmem_base_smem;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ntaps = g.KH * g.KW;
-  const int gid = blockIdx.x % g.ngroups;                           // which slice of the filter taps
-  const int tb = gid * g.taps_per_group, te = min(ntaps, tb + g.taps_per_group);
-  const int cta_in_group = blockIdx.x / g.ngroups, ctas_per_group = (gridDim.x + g.ngroups - 1 - gid) / g.ngroups;
-  const int ncols = (te - tb) * CBLK * 64;
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < (uint32_t)g.ncols_max) tmem_cols <<= 1;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&map_dout);
-    tma_prefetch_desc(&map_x);
-    for (int s = 0; s < kWgMaxStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);          // both issuers commit
-    }
-    mbar_init(&done_bar, 2);
-    fence_mbar_init();
-  }
-  if (warp == 1) w_tmem_alloc(&tmem_base_smem, tmem_cols);
-  w_fence_before();
-  __syncthreads();
-  w_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = cta_in_group; tile < g.num_tiles; tile += ctas_per_group, ++it) {
-        const uint32_t s = it % nstages;
-        mbar_wait(&empty_bar[s], ((it / nstages) & 1u) ^ 1u);
-        mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(kWgBM * 128 + CBLK * g.wrows * 128));
-        unsigned char* st = smem + s * stage_bytes;
-        tma_load_2d(st, &map_dout, 0, tile * kWgBM, &full_bar[s]);
-        for (int cb = 0; cb < CBLK; ++cb)
-          tma_load_2d(st + kWgBM * 128 + cb * win_bytes, &map_x, cb * 64, tile * kWgBM, &full_bar[s]);
-      }
-    }
-  } else if (warp == 1 || warp == 6) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = w_idesc_bf16_mn(64, 64);
-      // this issuer's taps of the group: local indices [j0, j0 + nmine)
-      const int ntg = te - tb, half = (ntg + 1) >> 1;
-      const int j0 = warp == 1 ? 0 : half, nmine = warp == 1 ? half : ntg - half;
-      uint32_t tap_off[kWgTapsPerIssuer];                    // window shift of each tap in 16-byte units
-#pragma unroll
-      for (int j = 0; j < kWgTapsPerIssuer; ++j) {
-        const int tap = tb + j0 + j, r = tap / g.KW;
-        tap_off[j] = (uint32_t)(r * g.W + tap - r * g.KW) * 8u;
-      }
-      const uint32_t lo0 = (smem_u32(smem) >> 4) + kWgLoLbo1, stage16 = (uint32_t)stage_bytes >> 4;
-      const uint32_t win16 = (uint32_t)win_bytes >> 4;
-      uint32_t s = 0, par = 0, acc0 = 0;
-      for (int tile = cta_in_group; tile < g.num_tiles; tile += ctas_per_group) {
-        mbar_wait(&full_bar[s], par);
-        w_fence_after();
-        const uint32_t a_lo = lo0 + s * stage16, x_lo = a_lo + (uint32_t)(kWgBM * 128 >> 4);
-#pragma unroll
-        for (int j = 0; j < kWgTapsPerIssuer; ++j) {
-          if (j < nmine) {
-#pragma unroll
-            for (int cb = 0; cb < CBLK; ++cb) {
-              const uint32_t d_tmem = tmem_base + (uint32_t)(((j0 + j) * CBLK + cb) * 64);
-              const uint32_t b_lo = x_lo + cb * win16 + tap_off[j];
-#pragma unroll
-              for (int kk = 0; kk < kWgBM / 16; ++kk)   // K advances by 16 positions = 16 rows of 128 bytes (128 units)
-                w_umma(d_tmem, w_desc(kWgHiSw128, a_lo + kk * 128u), w_desc(kWgHiSw128, b_lo + kk * 128u), idesc,
-                       kk == 0 ? acc0 : 1u);
-            }
-          }
-        }
-        w_commit(&empty_bar[s]);
-        acc0 = 1u;
-        if (++s == nstages) s = 0, par ^= 1u;
-      }
-      w_commit(&done_bar);
-    }
-  } else if (warp < 6) {
-    // ===== dump the TMEM accumulators once: [128 lanes][ncols] raw (the reduce kernel maps lanes -> rows) =====
-    const int qd = warp & 3;
-    mbar_wait(&done_bar, 0);
-    w_fence_after();
-    float* dst = g.partials + ((size_t)blockIdx.x * 128 + qd * 32 + lane) * g.ncols_max;
-    const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16);
-    for (int c0 = 0; c0 < ncols; c0 += 16) {
-      float v[16];
-      w_tmem_ld16(taddr + (uint32_t)c0, v);
-#pragma unroll
-      for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(dst + c0 + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-    }
-  }
-  w_fence_before();
-  __syncthreads();
-  if (warp == 1) w_tmem_dealloc(tmem_base, tmem_cols);
-}
-
-// dW[co][(tap, ci)] = sum over the CTAs of the tap's group, in CTA order (deterministic).
-// lane_map 0: accumulator row i of an M=64 tile lives in TMEM lane 32*(i/16) + i%16 ; 1: lane i.
-__global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float* __restrict__ partials, int nctas, int ngroups,
-                                                           int taps_per_group, int ntaps, int cblk, int ncols_max,
-                                                           int lane_map, float* __restrict__ dw, int accumulate) {
-  const int K = ntaps * cblk * 64;
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= 64 * K) return;
-  const int co = idx / K, k = idx - co * K;
-  const int tap = k / (cblk * 64), within = k - tap * cblk * 64;
-  const int gid = tap / taps_per_group;
-  const int col = (tap - gid * taps_per_group) * cblk * 64 + within;
-  const int ln = lane_map == 0 ? 32 * (co >> 4) + (co & 15) : co;
-  float acc = 0.f;
-  for (int c = gid; c < nctas; c += ngroups) acc += partials[((size_t)c * 128 + ln) * ncols_max + col];
-  dw[idx] = accumulate ? dw[idx] + acc : acc;
-}
-
-// Cout = 32 variant (conv1 of the Atari net): the roles are swapped so that the 64-byte dout rows become the
-// N = 32 operand:  D_t[ci, co] = sum_q in[q + off_t, ci] * dout[q, co];  A = input window (MN-major, SW128, M = 64),
-// B = dout tile (MN-major, SWIZZLE_64B, N = 32).  One group: KH*KW taps x 32 columns of TMEM.
-__global__ void __launch_bounds__(kWgThreads, 1) wgrad_window_n32_kernel(const __grid_constant__ CUtensorMap map_dout,
-                                                                         const __grid_constant__ CUtensorMap map_x,
-                                                                         const WgradArgs g) {
-  extern __shared__ __align__(1024) unsigned char smem_dyn[];
-  unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
-  const int win_bytes = (g.wrows * 128 + 1023) & ~1023;
-  const int stage_bytes = kWgBM * 64 + win_bytes;                    // 8 KB dout tile + input window
-  __shared__ __align__(8) unsigned long long full_bar[kWgMaxStages], empty_bar[kWgMaxStages], done_bar;
-  __shared__ uint32_t tmem_base_smem;
-  const uint32_t nstages = (uint32_t)g.stages;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ntaps = g.KH * g.KW;
-  const int ncols = ntaps * 32;
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < (uint32_t)ncols) tmem_cols <<= 1;
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&map_dout);
-    tma_prefetch_desc(&map_x);
-    for (int s = 0; s < kWgMaxStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);          // both issuers commit
-    }
-    mbar_init(&done_bar, 2);
-    fence_mbar_init();
-  }
-  if (warp == 1) w_tmem_alloc(&tmem_base_smem, tmem_cols);
-  w_fence_before();
-  __syncthreads();
-  w_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x, ++it) {
-        const uint32_t s = it % nstages;
-        mbar_wait(&empty_bar[s], ((it / nstages) & 1u) ^ 1u);
-        mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(kWgBM * 64 + g.wrows * 128));
-        unsigned char* st = smem + s * stage_bytes;
-        tma_load_2d(st + kWgBM * 64, &map_x, 0, tile * kWgBM, &full_bar[s]);     // window first: 1024-byte aligned
-        tma_load_2d(st, &map_dout, 0, tile * kWgBM, &full_bar[s]);
-      }
-    }
-  } else if (warp == 1 || warp == 6) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = w_idesc_bf16_mn(64, 32);
-      const int half = (ntaps + 1) >> 1;
-      const int j0 = warp == 1 ? 0 : half, nmine = warp == 1 ? half : ntaps - half;
-      uint32_t tap_off[kWgTapsPerIssuer];
-#pragma unroll
-      for (int j = 0; j < kWgTapsPerIssuer; ++j) {
-        const int tap = j0 + j, r = tap / g.KW;
-        tap_off[j] = (uint32_t)(r * g.W + tap - r * g.KW) * 8u;
-      }
-      const uint32_t lo0 = (smem_u32(smem) >> 4) + kWgLoLbo1, stage16 = (uint32_t)stage_bytes >> 4;
-      uint32_t s = 0, par = 0, acc0 = 0;
-      for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-        mbar_wait(&full_bar[s], par);
-        w_fence_after();
-        const uint32_t b_lo = lo0 + s * stage16;                              // dout tile, 64-byte rows
-        const uint32_t x_lo = b_lo + (uint32_t)(kWgBM * 64 >> 4);
-#pragma unroll
-        for (int j = 0; j < kWgTapsPerIssuer; ++j) {
-          if (j < nmine) {
-            const uint32_t a_lo = x_lo + tap_off[j];
-            const uint32_t d_tmem = tmem_base + (uint32_t)((j0 + j) * 32);
-#pragma unroll
-            for (int kk = 0; kk < kWgBM / 16; ++kk)     // 16 positions = 2048 B of window rows, 1024 B of dout rows
-              w_umma(d_tmem, w_desc(kWgHiSw128, a_lo + kk * 128u), w_desc(kWgHiSw64, b_lo + kk * 64u), idesc,
-                     kk == 0 ? acc0 : 1u);
-          }
-        }
-        w_commit(&empty_bar[s]);
-        acc0 = 1u;
-        if (++s == nstages) s = 0, par ^= 1u;
-      }
-      w_commit(&done_bar);
-    }
-  } else if (warp < 6) {
-    const int qd = warp & 3;
-    mbar_wait(&done_bar, 0);
-    w_fence_after();
-    float* dst = g.partials + ((size_t)blockIdx.x * 128 + qd * 32 + lane) * g.ncols_max;
-    const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16);
-    for (int c0 = 0; c0 < ncols; c0 += 16) {
-      float v[16];
-      w_tmem_ld16(taddr + (uint32_t)c0, v);
-#pragma unroll
-      for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(dst + c0 + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-    }
-  }
-  w_fence_before();
-  __syncthreads();
-  if (warp == 1) w_tmem_dealloc(tmem_base, tmem_cols);
-}
-
-// dW[co][(tap, ci)] (Cout = 32, Cin = 64) from the [ci lanes][tap*32 + co] partials, CTA order (deterministic)
-__global__ void __launch_bounds__(256) wgrad_reduce_n32_kernel(const float* __restrict__ partials, int nctas, int ntaps,
-                                                               int ncols_max, float* __restrict__ dw, int accumulate) {
-  const int K = ntaps * 64;
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= 32 * K) return;
-  const int co = idx / K, k = idx - co * K;
-  const int tap = k >> 6, ci = k & 63;
-  const int ln = 32 * (ci >> 4) + (ci & 15);
-  float acc = 0.f;
-  for (int c = 0; c < nctas; ++c) acc += partials[((size_t)c * 128 + ln) * ncols_max + tap * 32 + co];
-  dw[idx] = accumulate ? dw[idx] + acc : acc;
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------
-// Paired-tap form (default).  Roles swapped — A = input window (MN-major, SWIZZLE_128B), B = dout tile (MN-major;
-// SWIZZLE_128B for 64 output channels, SWIZZLE_64B for 32) — and TWO filter taps share one instruction: an
-// MN-major operand's second 64-element block lies LBO bytes after the first, and the windows of two taps are the
-// same rows shifted by (off_{t+1} - off_t) * 128 bytes, so LBO = that shift gives an M = 128 tile
-//     D[(tap_lo | tap_hi, ci), co] += in[q + off, ci]^T dout[q, co]
-// at the tensor-core cost of one M = 64 tile.  Half the instructions, all 128 TMEM lanes used, so every tap of a
-// 3x3 / 64-channel layer fits the 512 columns at once (5 pairs x 64) and no position tile is read by two CTA groups
-// (the M = 64 form read conv3's operands twice: ncu round 1, 11.9 GB for 6.3 GB of unique data).  An odd last tap
-// is paired with the window one row further down; its upper 64 lanes are never read back.
-// The bias gradient rides along: one more M = 64 instruction per K step whose A operand is a constant tile of ones,
-//     D_b[m, co] += sum_q 1 * dout[q, co]        (every row m holds the column sums; lane 0 is read back)
-// so the gradient grid is not streamed from HBM a second time by a column-sum kernel.
-// ---------------------------------------------------------------------------------------------------------------
-constexpr int kWgSlotsPerIssuer = 3;      // (pair, channel-block) accumulators per issuing warp
-
-struct WgradPairArgs {
-  float* partials;                    // [gridDim.x][128 lanes][ncols] raw TMEM dumps
+  float* partials;                    // [gridDim.x][per_group slots][64 rows][COUT]
   int W, KW, ntaps;
   int wrows, num_tiles, stages;
-  int npairs, ncols;                  // ncols = npairs * CBLK * COUT (+ 2 * COUT bias-gradient columns)
-  int bias;                           // 1: also accumulate the column sums of dout (bias gradient) in TMEM
+  int ngroups, per_group;             // slot s lives in group s / per_group; CTA b belongs to group b % ngroups
+  int bias;                           // 1: the last slot is the bias gradient (column sums of dout)
   float in_scale;                     // U8X: input operand = bf16(byte * in_scale)
 };
 
 // U8X (conv1 on the uint8 observation): map_x is the uint8 [Q][64] matrix; the producer fills a dense staging ring
-// and eight warps — the four dump warps (idle until the last tile) plus four extra ones (7-10) — convert each window
-// into the bf16 SWIZZLE_128B slot (u8win.cuh).
-constexpr int kWgU8Threads = kWgThreads + kU8Threads - 128;
-template <int COUT, int CBLK, bool U8X = false>
-__global__ void __launch_bounds__(U8X ? kWgU8Threads : kWgThreads, 1) wgrad_pair_kernel(const __grid_constant__ CUtensorMap map_dout,
-                                                                   const __grid_constant__ CUtensorMap map_x,
-                                                                   const WgradPairArgs g) {
+// and 256 more threads convert each window into the bf16 SWIZZLE_128B slot (u8win.cuh).
+// DOUT_A (rl_debug_set_wgrad_lane_map(2), Cout = 64, no bias slot): the operand roles swapped — A = dout tile
+// (M = 64 output channels), B = shifted input window (N = 64 input channels), accumulator rows = output channels —
+// an independent cross-check of the MN-major descriptors in both operand positions.
+template <int COUT, int CBLK, bool U8X = false, bool DOUT_A = false>
+__global__ void __launch_bounds__(U8X ? kWgThreads + kU8Threads : kWgThreads, 1)
+    wgrad_kernel(const __grid_constant__ CUtensorMap map_dout, const __grid_constant__ CUtensorMap map_x, const WgradArgs g) {
   static_assert(!U8X || CBLK == 1, "the uint8 window is one 64-channel block");
+  static_assert(!DOUT_A || (COUT == 64 && !U8X), "the swapped-role form is built for 64 output channels");
   constexpr int DOUT_BYTES = kWgBM * COUT * 2;                        // 16 KB (SW128) or 8 KB (SW64)
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   const int win_bytes = (g.wrows * 128 + 1023) & ~1023;
   const int stage_bytes = CBLK * win_bytes + DOUT_BYTES;              // windows first (1024-byte aligned), then dout
-  __shared__ __align__(8) unsigned long long full_bar[kWgMaxStages], empty_bar[kWgMaxStages], done_bar;
+  __shared__ __align__(8) unsigned long long full_bar[kWgMaxStages], empty_bar[kWgMaxStages];
   __shared__ __align__(8) unsigned long long u8_full[kU8Stages], u8_empty[kU8Stages];
-  __shared__ uint32_t tmem_base_smem;
   const uint32_t nstages = (uint32_t)g.stages;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < (uint32_t)g.ncols) tmem_cols <<= 1;
+  const int gid = blockIdx.x % g.ngroups;
+  const int cta_in_group = blockIdx.x / g.ngroups, ctas_per_group = (gridDim.x + g.ngroups - 1 - gid) / g.ngroups;
+  // constant A operand of the bias-gradient slot: 16 K-rows x 64 bf16 ones, after the stage ring
+  unsigned char* s_ones = smem + nstages * stage_bytes;
+  unsigned char* sStage = s_ones + 2048;                              // U8X: [kU8Stages][wrows][64 B]
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_dout);
     tma_prefetch_desc(&map_x);
     for (int s = 0; s < kWgMaxStages; ++s) {
       mbar_init(&full_bar[s], U8X ? 1 + kU8Threads : 1);   // U8X: the dout TMA + every converter thread
-      mbar_init(&empty_bar[s], 2);          // both issuers commit
+      mbar_init(&empty_bar[s], 2);                          // one arrival per consumer warpgroup
     }
     for (int s = 0; s < kU8Stages; ++s) {
       mbar_init(&u8_full[s], 1);
       mbar_init(&u8_empty[s], kU8Threads);
     }
-    mbar_init(&done_bar, 2);
     fence_mbar_init();
   }
-  if (warp == 1) w_tmem_alloc(&tmem_base_smem, tmem_cols);
-  // constant A operand of the bias-gradient instruction: 16 K-rows x 64 bf16 ones, after the stage ring
-  unsigned char* s_ones = smem + nstages * stage_bytes;
-  unsigned char* sStage = s_ones + 2048;                              // U8X: [kU8Stages][wrows][64 B]
   if (g.bias) {
-    for (int i = threadIdx.x; i < 512; i += kWgThreads) reinterpret_cast<uint32_t*>(s_ones)[i] = 0x3F803F80u;
+    for (int i = threadIdx.x; i < 512; i += blockDim.x) reinterpret_cast<uint32_t*>(s_ones)[i] = 0x3F803F80u;
     fence_proxy_async_smem();               // generic-proxy stores -> visible to the tensor core's async proxy
   }
-  w_fence_before();
   __syncthreads();
-  w_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (threadIdx.x < 128) {
+    if (threadIdx.x == 0) {
       uint32_t s = 0, par = 1, ss = 0, spar = 1;
       const int sbytes = u8_stage_bytes(g.wrows);
-      for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
+      for (int tile = cta_in_group; tile < g.num_tiles; tile += ctas_per_group) {
         if (U8X) {
           mbar_wait(&u8_empty[ss], spar);
           mbar_arrive_expect_tx(&u8_full[ss], (uint32_t)(g.wrows * 64));
@@ -424,122 +101,110 @@ __global__ void __launch_bounds__(U8X ? kWgU8Threads : kWgThreads, 1) wgrad_pair
         if (++s == nstages) s = 0, par ^= 1u;
       }
     }
-  } else if (warp == 1 || warp == 6) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = w_idesc_bf16_mn(128, COUT);
-      constexpr uint32_t hiB = COUT == 64 ? kWgHiSw128 : kWgHiSw64;
-      constexpr uint32_t kstepB = COUT == 64 ? 128u : 64u;             // 16 positions of dout rows, 16-byte units
-      // this issuer's accumulator slots: slot = pair * CBLK + cb, local indices [j0, j0 + nmine)
-      const int nslots = g.npairs * CBLK, half = (nslots + 1) >> 1;
-      const int j0 = warp == 1 ? 0 : half, nmine = warp == 1 ? half : nslots - half;
-      uint32_t a_off[kWgSlotsPerIssuer];      // (window shift of the pair's first tap + channel block) | LBO << 16
-#pragma unroll
-      for (int j = 0; j < kWgSlotsPerIssuer; ++j) {
-        const int slot = j0 + j, pair = slot / CBLK, cb = slot - pair * CBLK;
-        const int t0 = 2 * pair, t1 = min(2 * pair + 1, g.ntaps - 1);
-        const int r0 = t0 / g.KW, r1 = t1 / g.KW;
-        const int o0 = r0 * g.W + t0 - r0 * g.KW, o1 = r1 * g.W + t1 - r1 * g.KW;
-        const int delta = o1 > o0 ? o1 - o0 : 1;                       // odd last tap: dummy partner one row down
-        a_off[j] = (uint32_t)(o0 * 8 + cb * (win_bytes >> 4)) + ((uint32_t)(delta * 8) << 16);
-      }
-      const uint32_t lo0 = smem_u32(smem) >> 4, stage16 = (uint32_t)stage_bytes >> 4;
-      constexpr uint32_t idesc_bias = w_idesc_bf16_mn(64, COUT);
-      // bias gradient: each issuer takes every other K step into its OWN accumulator (no ordering between issuers)
-      const bool do_bias = g.bias != 0;
-      const uint32_t issuer = warp == 1 ? 0u : 1u;
-      const uint32_t ones_lo = (smem_u32(s_ones) >> 4) + kWgLoLbo1;
-      const uint32_t d_bias = tmem_base + (uint32_t)(nslots * COUT) + issuer * COUT;
-      uint32_t s = 0, par = 0, acc0 = 0;
-      for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-        mbar_wait(&full_bar[s], par);
-        w_fence_after();
-        const uint32_t x_lo = lo0 + s * stage16;
-        const uint32_t b_lo = x_lo + (uint32_t)((CBLK * win_bytes) >> 4) + kWgLoLbo1;
-#pragma unroll
-        for (int j = 0; j < kWgSlotsPerIssuer; ++j) {
-          if (j < nmine) {
-            const uint32_t d_tmem = tmem_base + (uint32_t)((j0 + j) * COUT);
-            const uint32_t a_lo = x_lo + a_off[j];
-#pragma unroll
-            for (int kk = 0; kk < kWgBM / 16; ++kk)       // 16 positions = 16 window rows (128 units) per K step
-              w_umma(d_tmem, w_desc(kWgHiSw128, a_lo + kk * 128u), w_desc(hiB, b_lo + kk * kstepB), idesc,
-                     kk == 0 ? acc0 : 1u);
-          }
-        }
-        if (do_bias) {
-#pragma unroll
-          for (int k2 = 0; k2 < kWgBM / 32; ++k2)
-            w_umma(d_bias, w_desc(kWgHiSw128, ones_lo), w_desc(hiB, b_lo + (2u * k2 + issuer) * kstepB), idesc_bias,
-                   k2 == 0 ? acc0 : 1u);
-        }
-        w_commit(&empty_bar[s]);
-        acc0 = 1u;
-        if (++s == nstages) s = 0, par ^= 1u;
-      }
-      w_commit(&done_bar);
-    }
-  } else {
-    // ===== dump the TMEM accumulators once: [128 lanes][ncols] =====
-    const int qd = warp & 3;
-    if (U8X) {
-      // uint8 -> bf16 window converters (these warps have nothing else to do until the accumulators are final)
-      const int ct = warp < 6 ? threadIdx.x - 64 : threadIdx.x - kWgThreads + 128;
-      const int sbytes = u8_stage_bytes(g.wrows);
-      const float cbias = -8388608.0f * g.in_scale;
-      uint32_t s = 0, epar = 1, ss = 0, fpar = 0;
-      for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-        mbar_wait(&u8_full[ss], fpar);
-        mbar_wait(&empty_bar[s], epar);            // the MMAs that read this slot have completed
-        w_fence_after();
-        u8_window_to_bf16_sw128(sStage + ss * sbytes, smem + s * stage_bytes, g.wrows, ct, g.in_scale, cbias);
-        fence_proxy_async_smem();
-        w_mbar_arrive(&full_bar[s]);
-        w_mbar_arrive(&u8_empty[ss]);
-        if (++s == nstages) s = 0, epar ^= 1u;
-        if (++ss == kU8Stages) ss = 0, fpar ^= 1u;
-      }
-    }
-    if (warp < 6) {
-      mbar_wait(&done_bar, 0);
-      w_fence_after();
-      float* dst = g.partials + ((size_t)blockIdx.x * 128 + qd * 32 + lane) * g.ncols;
-      const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16);
-      for (int c0 = 0; c0 < g.ncols; c0 += 16) {
-        float v[16];
-        w_tmem_ld16(taddr + (uint32_t)c0, v);
-#pragma unroll
-        for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4*>(dst + c0 + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-      }
-    }
+    return;
   }
-  w_fence_before();
-  __syncthreads();
-  if (warp == 1) w_tmem_dealloc(tmem_base, tmem_cols);
-}
-
-// dW[co][(tap, cb, ci)] from the [lane = (tap & 1) * 64 + ci][col = ((tap >> 1) * cblk + cb) * cout + co] partials,
-// summed over the CTAs in index order (deterministic); db[co] from lane 0 of the bias-gradient columns
-__global__ void __launch_bounds__(256) wgrad_pair_reduce_kernel(const float* __restrict__ partials, int nctas, int ntaps,
-                                                                int cblk, int cout, int ncols, float* __restrict__ dw,
-                                                                float* __restrict__ db, int accumulate) {
-  const int K = ntaps * cblk * 64;
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= cout * K) {
-    const int co = idx - cout * K;
-    if (db && co < cout) {
-      const int col = ((ntaps + 1) / 2) * cblk * cout + co;          // two accumulators (one per issuer): col, col + cout
-      float acc = 0.f;
-      for (int c = 0; c < nctas; ++c) acc += partials[(size_t)c * 128 * ncols + col] + partials[(size_t)c * 128 * ncols + col + cout];
-      db[co] = accumulate ? db[co] + acc : acc;
+  if (U8X && threadIdx.x >= kWgThreads) {
+    // uint8 -> bf16 window converters
+    const int ct = threadIdx.x - kWgThreads;
+    const int sbytes = u8_stage_bytes(g.wrows);
+    const float cbias = -8388608.0f * g.in_scale;
+    uint32_t s = 0, epar = 1, ss = 0, fpar = 0;
+    for (int tile = cta_in_group; tile < g.num_tiles; tile += ctas_per_group) {
+      mbar_wait(&u8_full[ss], fpar);
+      mbar_wait(&empty_bar[s], epar);            // the MMAs that read this slot have completed
+      u8_window_to_bf16_sw128(sStage + ss * sbytes, smem + s * stage_bytes, g.wrows, ct, g.in_scale, cbias);
+      fence_proxy_async_smem();
+      mbar_arrive(&full_bar[s]);
+      mbar_arrive(&u8_empty[ss]);
+      if (++s == nstages) s = 0, epar ^= 1u;
+      if (++ss == kU8Stages) ss = 0, fpar ^= 1u;
     }
     return;
   }
-  const int co = idx / K, k = idx - co * K;
-  const int tap = k / (cblk * 64), within = k - tap * cblk * 64, cb = within >> 6, ci = within & 63;
-  const int ln = (tap & 1) * 64 + ci, col = ((tap >> 1) * cblk + cb) * cout + co;
+  // ===== consumers: warpgroup c owns local slots [j0, j0 + nmine) of this CTA's group =====
+  const int c = (threadIdx.x >> 7) - 1, t = threadIdx.x & 127;
+  const int nslots_all = g.ntaps * CBLK + g.bias;
+  const int gs0 = gid * g.per_group, ngs = min(g.per_group, nslots_all - gs0);
+  const int half = (ngs + 1) >> 1, j0 = c == 0 ? 0 : half, nmine = c == 0 ? half : ngs - half;
+  constexpr uint32_t hiB = COUT == 64 ? kGmmaHiSw128 : kGmmaHiSw64;
+  constexpr uint32_t kstepB = COUT == 64 ? 128u : 64u;               // 16 positions of dout rows, 16-byte units
+  // Both warpgroups issue `half` MMA chains (a bound that does not depend on the thread index, so the wgmma stay
+  // warpgroup-uniform and are not serialised); when ngs is odd the second warpgroup's last chain is a dummy that reads
+  // the ones tile and is never written back.
+  uint32_t a_off[kWgSlots];        // per slot: window shift + channel block (16-byte units), or the ones tile
+  bool is_ones[kWgSlots];
+#pragma unroll
+  for (int j = 0; j < kWgSlots; ++j) {
+    const int slot = gs0 + j0 + j;
+    is_ones[j] = slot >= g.ntaps * CBLK || j >= nmine;
+    const int tap = slot / CBLK, cb = slot - tap * CBLK, r = tap / g.KW;
+    a_off[j] = is_ones[j] ? 0u : (uint32_t)((r * g.W + tap - r * g.KW) * 8 + cb * (win_bytes >> 4));
+  }
+  const uint32_t lo0 = gmma_lo(smem), stage16 = (uint32_t)stage_bytes >> 4, ones_lo = gmma_lo(s_ones);
+  float d[kWgSlots][COUT / 2];
+#pragma unroll
+  for (int j = 0; j < kWgSlots; ++j)
+#pragma unroll
+    for (int i = 0; i < COUT / 2; ++i) d[j][i] = 0.f;
+  uint32_t s = 0, par = 0;
+  for (int tile = cta_in_group; tile < g.num_tiles; tile += ctas_per_group) {
+    mbar_wait(&full_bar[s], par);
+    wgmma_fence();
+    const uint32_t x_lo = lo0 + s * stage16;
+    const uint32_t b_lo = x_lo + (uint32_t)((CBLK * win_bytes) >> 4);
+#pragma unroll
+    for (int j = 0; j < kWgSlots; ++j) {
+      if (j < half) {
+#pragma unroll
+        for (int kk = 0; kk < kWgBM / 16; ++kk) {   // 16 positions = 16 window rows (128 units) per K step
+          const uint32_t a_lo = is_ones[j] ? ones_lo : x_lo + a_off[j] + kk * 128u;
+          if constexpr (DOUT_A)
+            wgmma_bf16<COUT, 1, 1>(d[j], gmma_desc(kGmmaHiSw128, b_lo + kk * kstepB), gmma_desc(kGmmaHiSw128, a_lo), 1u);
+          else
+            wgmma_bf16<COUT, 1, 1>(d[j], gmma_desc(kGmmaHiSw128, a_lo), gmma_desc(hiB, b_lo + kk * kstepB), 1u);
+        }
+      }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (t == 0) mbar_arrive(&empty_bar[s]);
+    if (++s == nstages) s = 0, par ^= 1u;
+  }
+#pragma unroll
+  for (int j = 0; j < kWgSlots; ++j) {
+    wgmma_fence_regs(d[j]);
+    if (j < nmine) {
+      float* dst = g.partials + ((size_t)blockIdx.x * g.per_group + j0 + j) * 64 * COUT;
+#pragma unroll
+      for (int i = 0; i < COUT / 2; i += 2)
+        *reinterpret_cast<float2*>(dst + gmma_row(t, i) * COUT + gmma_col(t, i)) = make_float2(d[j][i], d[j][i + 1]);
+    }
+  }
+}
+
+// dW[co][(tap, cb, ci)] = sum over the CTAs of the slot's group in index order (deterministic); db[co] from row 0 of
+// the bias slot.  dout_rows: the partial tiles are [co][ci] (swapped-role form) instead of [ci][co].
+__global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float* __restrict__ partials, int nctas, int ngroups,
+                                                           int per_group, int ntaps, int cblk, int cout, int dout_rows,
+                                                           float* __restrict__ dw, float* __restrict__ db, int accumulate) {
+  const int K = ntaps * cblk * 64;
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  int slot, row, co;
+  if (idx >= cout * K) {
+    co = idx - cout * K;
+    if (!db || co >= cout) return;
+    slot = ntaps * cblk, row = 0;
+  } else {
+    co = idx / K;
+    const int k = idx - co * K;
+    slot = k >> 6, row = k & 63;                        // k = (tap * cblk + cb) * 64 + ci
+  }
+  const int gid = slot / per_group, local = slot - gid * per_group;
   float acc = 0.f;
-  for (int c = 0; c < nctas; ++c) acc += partials[((size_t)c * 128 + ln) * ncols + col];
-  dw[idx] = accumulate ? dw[idx] + acc : acc;
+  const size_t off = dout_rows ? (size_t)co * 64 + row : (size_t)row * cout + co;
+  for (int c = gid; c < nctas; c += ngroups) acc += partials[((size_t)c * per_group + local) * 64 * cout + off];
+  if (idx >= cout * K) db[co] = accumulate ? db[co] + acc : acc;
+  else dw[idx] = accumulate ? dw[idx] + acc : acc;
 }
 
 // column sums of a [rows, C] bf16 matrix (bias gradients): deterministic two-stage, 16-byte loads.
@@ -623,27 +288,33 @@ static int wg_make_map(CUtensorMap* map, const void* base, uint64_t cols, uint64
 
 using namespace rl;
 
-// bit 0: legacy M = 64 kernels read accumulator row i from TMEM lane i (wrong on B200; the measured map is
-// 32*(i/16) + i%16) — triage only.  bit 1: use the legacy one-tap-per-instruction (M = 64) kernels instead of the
-// paired-tap form.
-static int g_wg_lane_map = 0;
+// Weight-gradient form.  0 (default): A = input window, B = dout, bias gradient as a slot against a tile of ones;
+// 2: for 64 output channels the operand roles swapped (wgrad_kernel<64, CBLK, false, true>), and the bias gradient from
+// rl_colsum_bf16 — a cross-check of the default form (Cout = 32 keeps the default roles, the uint8 input the default form).
+static int g_wg_form = 0;
 extern "C" int rl_debug_set_wgrad_lane_map(int mode) {
-  g_wg_lane_map = mode;
+  RL_CHECK_ARG(mode == 0 || mode == 2, "wgrad form must be 0 (default) or 2 (swapped operand roles)");
+  g_wg_form = mode;
   return RL_OK;
 }
 
-extern "C" size_t rl_conv_wgrad_workspace_bytes(int KH, int KW, int Cin) {
-  const int cblk = Cin / 64, ntaps = KH * KW;
-  int per = 512 / (cblk * 64);
-  if (per > ntaps) per = ntaps;
-  return (size_t)160 * 128 * (size_t)(per * cblk * 64) * sizeof(float) + 4096;
+static void wgrad_groups(int ntaps, int cblk, int bias, int* ngroups, int* per_group) {
+  const int nslots = ntaps * cblk + bias;
+  *ngroups = (nslots + 2 * kWgSlots - 1) / (2 * kWgSlots);
+  *per_group = (nslots + *ngroups - 1) / *ngroups;
 }
 
-static int wgrad_legacy_bias(const void* dout_grid, long long Q, int Cout, float* db, int accumulate, void* workspace,
-                             size_t workspace_bytes, rl_stream_t stream) {
-  if (!db) return RL_OK;
-  RL_CHECK_ARG(!accumulate, "conv2d_s1_wgrad: accumulate with a bias gradient needs the paired-tap form");
-  return rl_colsum_bf16(dout_grid, Q, Cout, db, workspace, workspace_bytes, stream);
+// Enough for every call with these filter dimensions: with or without the bias-gradient slot (the slot count, and so
+// the slots per CTA group, differ), either form, and the column-sum pass of form 2 (rl_colsum_bf16: 1184 x Cout floats).
+extern "C" size_t rl_conv_wgrad_workspace_bytes(int KH, int KW, int Cin) {
+  size_t need = (size_t)1184 * 64 * sizeof(float);
+  for (int bias = 0; bias <= 1; ++bias) {
+    int ngroups = 1, per = 1;
+    wgrad_groups(KH * KW, Cin / 64, bias, &ngroups, &per);
+    const size_t b = (size_t)kWgMaxCtas * per * 64 * 64 * sizeof(float);
+    if (b > need) need = b;
+  }
+  return need + 4096;
 }
 
 static int wgrad_dispatch(const void* dout_grid, const void* in, float* dw_krsc, float* db, int N, int H, int W, int Cin,
@@ -656,136 +327,73 @@ static int wgrad_dispatch(const void* dout_grid, const void* in, float* dw_krsc,
   const long long Q = (long long)N * H * W;
   RL_CHECK_ARG(Q < (1LL << 31), "conv2d_s1_wgrad: too many positions");
   const int cblk = Cin / 64, ntaps = KH * KW;
-  WgradArgs g;
-  g.partials = reinterpret_cast<float*>(workspace);
-  g.W = W, g.KH = KH, g.KW = KW, g.Q = (int)Q;
-  g.wrows = kWgBM + (KH - 1) * W + (KW - 1);
-  RL_CHECK_ARG(g.wrows <= 256, "conv2d_s1_wgrad: window too tall");
-  g.num_tiles = (int)((Q + kWgBM - 1) / kWgBM);
-  const int npairs = (ntaps + 1) / 2;
-  if (u8in || (!(g_wg_lane_map & 2) && npairs * cblk <= 2 * kWgSlotsPerIssuer && npairs * cblk * Cout <= 512)) {
-    // ---- paired-tap form (default) ----
-    WgradPairArgs a;
-    a.partials = reinterpret_cast<float*>(workspace);
-    a.W = W, a.KW = KW, a.ntaps = ntaps, a.wrows = g.wrows + 1;       // + the dummy partner row of an odd last tap
-    a.num_tiles = g.num_tiles, a.npairs = npairs, a.bias = db ? 1 : 0, a.in_scale = in_scale;
-    a.ncols = npairs * cblk * Cout + (db ? 2 * Cout : 0);            // + one bias accumulator per issuer
-    RL_CHECK_ARG(a.ncols <= 512, "conv2d_s1_wgrad: accumulators exceed the 512 TMEM columns");
-    RL_CHECK_ARG(a.wrows <= 256, "conv2d_s1_wgrad: window too tall");
-    int devp = 0, smsp = 148;
-    cudaGetDevice(&devp);
-    cudaDeviceGetAttribute(&smsp, cudaDevAttrMultiProcessorCount, devp);
-    smsp = effective_sms(smsp);
-    const int gridp = smsp < a.num_tiles ? smsp : a.num_tiles;
-    if (workspace_bytes < (size_t)gridp * 128 * a.ncols * sizeof(float)) {
-      set_error("conv2d_s1_wgrad: workspace too small");
-      return RL_ERR_WORKSPACE;
-    }
-    alignas(64) CUtensorMap mdp, mxp;
-    if (wg_make_map(&mdp, dout_grid, (uint64_t)Cout, (uint64_t)Q, kWgBM, (uint32_t)Cout,
-                    Cout == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B) ||
-        (u8in ? make_tensor_map_u8_rows64(&mxp, in, (uint64_t)Q, (uint32_t)a.wrows)
-              : wg_make_map(&mxp, in, (uint64_t)Cin, (uint64_t)Q, (uint32_t)a.wrows))) {
-      set_error("conv2d_s1_wgrad: cuTensorMapEncodeTiled failed");
-      return RL_ERR_CUDA;
-    }
-    const size_t winp = (size_t)((a.wrows * 128 + 1023) & ~1023);
-    const size_t stagep = (size_t)cblk * winp + (size_t)kWgBM * Cout * 2;
-    const size_t u8ring = u8in ? (size_t)kU8Stages * (size_t)((a.wrows * 64 + 1023) & ~1023) : 0;
-    long long nstp = (long long)((216 * 1024 - u8ring) / stagep);
-    a.stages = (int)(nstp > kWgMaxStages ? kWgMaxStages : (nstp < 2 ? 2 : nstp));
-    const size_t smemp = (size_t)a.stages * stagep + 2048 + 1024 + u8ring;   // + the 2 KB tile of ones (+ uint8 staging)
-    cudaStream_t stp = (cudaStream_t)stream;
-    if (u8in) {
-      auto kern = wgrad_pair_kernel<32, 1, true>;
-      RL_SMEM_OPTIN(kern);
-      kern<<<gridp, kWgU8Threads, smemp, stp>>>(mdp, mxp, a);
-    } else if (Cout == 64 && cblk == 1) {
-      RL_SMEM_OPTIN(wgrad_pair_kernel<64, 1>);
-      wgrad_pair_kernel<64, 1><<<gridp, kWgThreads, smemp, stp>>>(mdp, mxp, a);
-    } else if (Cout == 64) {
-      RL_SMEM_OPTIN(wgrad_pair_kernel<64, 2>);
-      wgrad_pair_kernel<64, 2><<<gridp, kWgThreads, smemp, stp>>>(mdp, mxp, a);
-    } else {
-      RL_SMEM_OPTIN(wgrad_pair_kernel<32, 1>);
-      wgrad_pair_kernel<32, 1><<<gridp, kWgThreads, smemp, stp>>>(mdp, mxp, a);
-    }
-    const int Kp = ntaps * cblk * 64;
-    wgrad_pair_reduce_kernel<<<(Cout * Kp + Cout + 255) / 256, 256, 0, stp>>>(a.partials, gridp, ntaps, cblk, Cout,
-                                                                             a.ncols, dw_krsc, db, accumulate);
-    RL_CHECK_LAUNCH("rl_conv2d_s1_nhwc_bf16_wgrad");
-    return RL_OK;
-  }
-  if (Cout == 32) {
-    // swapped-role variant: D[ci, co], dout rows are 64 bytes (SWIZZLE_64B operand)
-    RL_CHECK_ARG(ntaps <= 2 * kWgTapsPerIssuer, "conv2d_s1_wgrad: too many taps for Cout = 32");
-    g.ngroups = 1, g.taps_per_group = ntaps, g.ncols_max = ntaps * 32;
-    int dev32 = 0, sms32 = 148;
-    cudaGetDevice(&dev32);
-    cudaDeviceGetAttribute(&sms32, cudaDevAttrMultiProcessorCount, dev32);
-    sms32 = effective_sms(sms32);
-    int grid32 = sms32 < g.num_tiles ? sms32 : g.num_tiles;
-    if (workspace_bytes < (size_t)grid32 * 128 * g.ncols_max * sizeof(float)) {
-      set_error("conv2d_s1_wgrad: workspace too small");
-      return RL_ERR_WORKSPACE;
-    }
-    alignas(64) CUtensorMap md32, mx32;
-    if (wg_make_map(&md32, dout_grid, 32, (uint64_t)Q, kWgBM, 32, CU_TENSOR_MAP_SWIZZLE_64B) ||
-        wg_make_map(&mx32, in, 64, (uint64_t)Q, (uint32_t)g.wrows)) {
-      set_error("conv2d_s1_wgrad: cuTensorMapEncodeTiled failed");
-      return RL_ERR_CUDA;
-    }
-    const size_t win32 = (size_t)((g.wrows * 128 + 1023) & ~1023);
-    long long nst32 = (long long)((218 * 1024) / (kWgBM * 64 + win32));
-    g.stages = (int)(nst32 > kWgMaxStages ? kWgMaxStages : (nst32 < 2 ? 2 : nst32));
-    const size_t smem32 = (size_t)g.stages * (kWgBM * 64 + win32) + 1024;
-    RL_SMEM_OPTIN(wgrad_window_n32_kernel);
-    wgrad_window_n32_kernel<<<grid32, kWgThreads, smem32, (cudaStream_t)stream>>>(md32, mx32, g);
-    wgrad_reduce_n32_kernel<<<(32 * ntaps * 64 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
-        g.partials, grid32, ntaps, g.ncols_max, dw_krsc, accumulate);
-    RL_CHECK_LAUNCH("rl_conv2d_s1_nhwc_bf16_wgrad");
-    return wgrad_legacy_bias(dout_grid, Q, Cout, db, accumulate, workspace, workspace_bytes, stream);
-  }
-  int cap = 512 / (cblk * 64);                       // taps whose accumulators fit the 512 TMEM columns
-  if (cap > ntaps) cap = ntaps;
-  g.ngroups = (ntaps + cap - 1) / cap;
-  g.taps_per_group = (ntaps + g.ngroups - 1) / g.ngroups;   // balanced split (e.g. 9 taps -> 5 + 4)
-  g.ncols_max = g.taps_per_group * cblk * 64;
-  RL_CHECK_ARG(g.taps_per_group <= 2 * kWgTapsPerIssuer, "conv2d_s1_wgrad: too many taps per CTA group");
-  int dev = 0, sms = 148;
+  WgradArgs a;
+  a.partials = reinterpret_cast<float*>(workspace);
+  a.W = W, a.KW = KW, a.ntaps = ntaps, a.wrows = kWgBM + (KH - 1) * W + (KW - 1);
+  RL_CHECK_ARG(a.wrows <= 256, "conv2d_s1_wgrad: window too tall");
+  const bool legacy = g_wg_form == 2 && !u8in;
+  RL_CHECK_ARG(!(legacy && db && accumulate), "conv2d_s1_wgrad: accumulate with a bias gradient needs the default form");
+  a.num_tiles = (int)((Q + kWgBM - 1) / kWgBM), a.bias = (db && !legacy) ? 1 : 0, a.in_scale = in_scale;
+  wgrad_groups(ntaps, cblk, a.bias, &a.ngroups, &a.per_group);
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   sms = effective_sms(sms);
-  int grid = sms;
-  if (grid > g.num_tiles * g.ngroups) grid = g.num_tiles * g.ngroups;
-  if (grid < g.ngroups) grid = g.ngroups;
-  if (workspace_bytes < (size_t)grid * 128 * g.ncols_max * sizeof(float)) {
+  // CTAs per group: one per position tile at most; the whole grid at most one per SM (and kWgMaxCtas)
+  long long per_grp = (sms < kWgMaxCtas ? sms : kWgMaxCtas) / a.ngroups;
+  if (per_grp < 1) per_grp = 1;
+  if (per_grp > a.num_tiles) per_grp = a.num_tiles;
+  const int grid = (int)per_grp * a.ngroups;
+  if (workspace_bytes < (size_t)grid * a.per_group * 64 * Cout * sizeof(float)) {
     set_error("conv2d_s1_wgrad: workspace too small");
     return RL_ERR_WORKSPACE;
   }
   alignas(64) CUtensorMap md, mx;
-  if (wg_make_map(&md, dout_grid, (uint64_t)Cout, (uint64_t)Q, kWgBM) ||
-      wg_make_map(&mx, in, (uint64_t)Cin, (uint64_t)Q, (uint32_t)g.wrows)) {
+  if (wg_make_map(&md, dout_grid, (uint64_t)Cout, (uint64_t)Q, kWgBM, (uint32_t)Cout,
+                  Cout == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B) ||
+      (u8in ? make_tensor_map_u8_rows64(&mx, in, (uint64_t)Q, (uint32_t)a.wrows)
+            : wg_make_map(&mx, in, (uint64_t)Cin, (uint64_t)Q, (uint32_t)a.wrows))) {
     set_error("conv2d_s1_wgrad: cuTensorMapEncodeTiled failed");
     return RL_ERR_CUDA;
   }
-  const size_t win = (size_t)((g.wrows * 128 + 1023) & ~1023);
-  long long nst = (long long)((218 * 1024) / (kWgBM * 128 + cblk * win));
-  g.stages = (int)(nst > kWgMaxStages ? kWgMaxStages : (nst < 2 ? 2 : nst));
-  const size_t smem = (size_t)g.stages * (kWgBM * 128 + cblk * win) + 1024;
+  const size_t win = (size_t)((a.wrows * 128 + 1023) & ~1023);
+  const size_t stage = (size_t)cblk * win + (size_t)kWgBM * Cout * 2;
+  const size_t u8ring = u8in ? (size_t)kU8Stages * (size_t)((a.wrows * 64 + 1023) & ~1023) : 0;
+  const long long nst = (long long)((216 * 1024 - u8ring) / stage);
+  a.stages = (int)(nst > kWgMaxStages ? kWgMaxStages : (nst < 2 ? 2 : nst));
+  const size_t smem = (size_t)a.stages * stage + 2048 + 1024 + u8ring;   // + the 2 KB tile of ones (+ uint8 staging)
   cudaStream_t st = (cudaStream_t)stream;
-  if (cblk == 1) {
-    RL_SMEM_OPTIN(wgrad_window_kernel<1>);
-    wgrad_window_kernel<1><<<grid, kWgThreads, smem, st>>>(md, mx, g);
+  if (u8in) {
+    RL_CHECK_ARG(Cout == 32 && cblk == 1, "conv2d_s1_u8in_wgrad: Cout 32, Cin 64");
+    auto kern = wgrad_kernel<32, 1, true>;
+    RL_SMEM_OPTIN(kern);
+    kern<<<grid, kWgThreads + kU8Threads, smem, st>>>(md, mx, a);
+  } else if (legacy && Cout == 64 && cblk == 1) {
+    auto kern = wgrad_kernel<64, 1, false, true>;
+    RL_SMEM_OPTIN(kern);
+    kern<<<grid, kWgThreads, smem, st>>>(md, mx, a);
+  } else if (legacy && Cout == 64) {
+    auto kern = wgrad_kernel<64, 2, false, true>;
+    RL_SMEM_OPTIN(kern);
+    kern<<<grid, kWgThreads, smem, st>>>(md, mx, a);
+  } else if (Cout == 64 && cblk == 1) {
+    RL_SMEM_OPTIN(wgrad_kernel<64, 1>);
+    wgrad_kernel<64, 1><<<grid, kWgThreads, smem, st>>>(md, mx, a);
+  } else if (Cout == 64) {
+    RL_SMEM_OPTIN(wgrad_kernel<64, 2>);
+    wgrad_kernel<64, 2><<<grid, kWgThreads, smem, st>>>(md, mx, a);
   } else {
-    RL_SMEM_OPTIN(wgrad_window_kernel<2>);
-    wgrad_window_kernel<2><<<grid, kWgThreads, smem, st>>>(md, mx, g);
+    RL_SMEM_OPTIN(wgrad_kernel<32, 1>);
+    wgrad_kernel<32, 1><<<grid, kWgThreads, smem, st>>>(md, mx, a);
   }
   const int K = ntaps * cblk * 64;
-  wgrad_reduce_kernel<<<(64 * K + 255) / 256, 256, 0, st>>>(g.partials, grid, g.ngroups, g.taps_per_group, ntaps, cblk,
-                                                           g.ncols_max, g_wg_lane_map & 1, dw_krsc, accumulate);
+  wgrad_reduce_kernel<<<(Cout * K + Cout + 255) / 256, 256, 0, st>>>(a.partials, grid, a.ngroups, a.per_group, ntaps, cblk,
+                                                                     Cout, legacy && Cout == 64 ? 1 : 0, dw_krsc,
+                                                                     a.bias ? db : nullptr, accumulate);
   RL_CHECK_LAUNCH("rl_conv2d_s1_nhwc_bf16_wgrad");
-  return wgrad_legacy_bias(dout_grid, Q, Cout, db, accumulate, workspace, workspace_bytes, stream);
+  // swapped-role form: the bias gradient by a column-sum pass (the partials are consumed: the workspace is free again)
+  if (db && !a.bias) return rl_colsum_bf16(dout_grid, Q, Cout, db, workspace, workspace_bytes, stream);
+  return RL_OK;
 }
 
 extern "C" int rl_conv2d_s1_nhwc_bf16_wgrad(const void* dout_grid, const void* in, float* dw_krsc, float* db, int N,

@@ -1,4 +1,4 @@
-"""A2C on one B200 — the on-device replacement of benchmark/torch/a2c/{train.py:33-177, actor.py:30-123}
+"""A2C on one H100 — the on-device replacement of benchmark/torch/a2c/{train.py:33-177, actor.py:30-123}
 (BASELINE configs[1]: 256 vectorised CartPole envs, fused GAE + policy-gradient kernels).
 
     rollout  ONE launch (rl_rollout_mlp): T lock-step steps of all B envs — actor-critic forward, exact categorical

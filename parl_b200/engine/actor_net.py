@@ -1,4 +1,4 @@
-"""Actor-side inference of the Atari actor-critic entirely on hand-written tcgen05 kernels
+"""Actor-side inference of the Atari actor-critic entirely on hand-written wgmma kernels
 (rl_conv2d_s1_nhwc_bf16_fwd x3 in TMA-window form + rl_gemm_bf16_tn x2): the policy forward the reference runs on CPU, batch 5,
 inside every remote actor (examples/IMPALA/actor.py:60-62, atari_agent.py:35-42) — here once per time
 step for the whole pool, reading the space-to-depth observation written by rl_obs_stack_gather and writing
@@ -23,10 +23,8 @@ class AtariActorNet(object):
         dev = self.device = torch.device(device)
         bf = torch.bfloat16
         self.window_form = window_form
-        # fc + policy head in one call (rl_gemm_bf16_tn_heads): the head is a warp-level mma.sync kernel instead of a
-        # tcgen05 GEMM whose 7-8 us are all prologue — rollout of 512 envs 2.55 vs 2.65 ms, neutral at 4096
-        # (profiles/r02_chain_ab.txt; the first attempt, a warp-per-row CUDA-core head fused into the split-K reduce,
-        # was slower: 3.04 ms)
+        # fc + policy head in one call (rl_gemm_bf16_tn_heads): the head (N2 = 18) is a warp-level mma.sync kernel
+        # instead of a tensor-core GEMM tile whose run time would be all prologue at that width
         self.fuse_heads = os.environ.get('PARL_B200_FUSE_HEADS', '1') != '0'
         # window form: conv1 writes conv2's zero-padded 2x2-block input [B,12,12,128] (border stays zero)
         self.a1 = (torch.zeros((self.B, 12, 12, 128), dtype=bf, device=dev) if window_form else

@@ -1,4 +1,4 @@
-"""DQN / DDQN with an HBM-resident (prioritised) Atari frame replay on one B200 — the on-device replacement of
+"""DQN / DDQN with an HBM-resident (prioritised) Atari frame replay on one H100 — the on-device replacement of
 benchmark/torch/dqn/{train.py:50-174, replay_memory.py:22-113, agent.py:57-104} with the proportional PER of
 benchmark/fluid/Prioritized_DQN/{proportional_per.py:18-157, per_alg.py:48-69} (BASELINE configs[4]: 1 M-transition
 HBM replay, priority sample + TD loss, sharded over the GPUs).

@@ -1,4 +1,4 @@
-"""The IMPALA actor-learner loop on one B200 (one process per GPU): the on-device replacement of
+"""The IMPALA actor-learner loop on one H100 (one process per GPU): the on-device replacement of
 examples/IMPALA/{train.py:34-252, actor.py:27-105} + the xparl RPC data path
 (parl/remote/remote_wrapper.py:178-227).
 
@@ -62,9 +62,10 @@ class ImpalaEngine(object):
         self.learner_sms = int(env_l) if env_l else (learner_sms or 0)
         if pipeline and actor_sms is None and learner_sms is None and not env_a and not env_l and int(num_envs) <= 768:
             # small per-GPU pools (the 8-GPU share of the 4096-actor workload): both streams' kernels are short and
-            # latency-bound, co-residency beats whole-GPU grids — measured at 512 envs on one B200 (tools/gpu_job8.sh):
-            # 6.33 ms per step uncapped, 5.74 ms at (74, 74), 5.68 ms at (64, 84); no gain at >= 1024 envs
-            self.actor_sms, self.learner_sms = 64, 84
+            # latency-bound, so the 132 SMs of an H100 are split between them and their kernels co-reside instead of
+            # serialising whole-GPU grids.  (57, 75) rescales the split measured on a 148-SM GPU to 132 SMs; it has
+            # not been measured on H100 (the actor_sms / learner_sms arguments override it)
+            self.actor_sms, self.learner_sms = 57, 75
         if role != 'both':
             assert not pipeline, 'actor-only / learner-only engines are driven through the host contract'
         self.B, self.T, self.A = int(num_envs), int(sample_batch_steps), int(act_dim)
@@ -89,9 +90,7 @@ class ImpalaEngine(object):
         self.stats = kernels.EpisodeStats(B, dev)
         self.s2d = (self.h, self.w) == (84, 84)              # conv1 space-to-depth input [N,21,21,64]
         # 'uint8' (default): the observation plane stays uint8 (half the bytes, 5.8 GB less per buffer set) and the
-        # conv1 kernels widen it to bf16 in shared memory; 'bf16': the gather pre-scales to bf16.  Measured on one B200,
-        # interleaved A/B at 4096 envs: step 36.4 / 36.8 ms (uint8) vs 36.9 / 37.0 ms (bf16); conv1 forward itself is
-        # 2 % slower at the learner batch (it is bound by the shared-memory data pipe, not by HBM), the gather 37 % faster.
+        # conv1 kernels widen it to bf16 in shared memory; 'bf16': the gather pre-scales to bf16.
         if obs_dtype is None:
             obs_dtype = os.environ.get('PARL_B200_OBS_DTYPE', 'uint8')
         obs_shape = (21, 21, 64) if self.s2d else (self.h, self.w, 4)
@@ -109,7 +108,7 @@ class ImpalaEngine(object):
         self.learn_chunk_rows = int(learn_chunk_rows)
         native_ok = (self.h, self.w) == (84, 84) and isinstance(self.model, AtariActorCritic)
         use_native_learner = role != 'actor' and (learner_kernels is True or (learner_kernels == 'auto' and native_ok))
-        # learner forward+backward on hand-written tcgen05 kernels (no autograd) when the model is the Atari net
+        # learner forward+backward on hand-written wgmma kernels (no autograd) when the model is the Atari net
         self.train_net = AtariTrainNet(self.model, T * B, dev, obs_dtype=self.obs_dtype if self.s2d else torch.bfloat16,
                                        flat=self._flat_master()) \
             if use_native_learner else None
@@ -123,7 +122,7 @@ class ImpalaEngine(object):
             self.values = torch.empty((T, B), dtype=torch.float32, device=dev)
             self.loss_out = dict(losses=torch.zeros(8, device=dev), d_logits=torch.empty((T * B, A), device=dev),
                                  d_values=torch.empty(T * B, device=dev))
-        # actor-side policy forward: hand-written tcgen05 conv/GEMM kernels when the model is the Atari
+        # actor-side policy forward: hand-written wgmma conv/GEMM kernels when the model is the Atari
         # actor-critic on 84x84 frames ('auto'), else the user's torch Model
         use_native = role != 'learner' and (actor_kernels is True or (actor_kernels == 'auto' and self.s2d and
                                                                      isinstance(self.model, AtariActorCritic)))
@@ -367,9 +366,7 @@ class ImpalaEngine(object):
         return res['losses'].clone()
 
     def _learn_native(self, learning_rate, entropy_coeff):
-        """learn() with the network forward/backward on the hand-written kernels (AtariTrainNet).  (Replaying the
-        update as CUDA graphs was measured at the 4- and 8-GPU shares of the workload — 5.23 vs 5.20 ms per step at 512
-        envs, 9.93 vs 9.86 at 1024, profiles/r02_learn_graph_ab.txt: the learner is not launch-bound — and removed.)"""
+        """learn() with the network forward/backward on the hand-written kernels (AtariTrainNet), launched eagerly."""
         res = self._learn_fwd_bwd(entropy_coeff)
         if self.alg.grad_sync is not None:
             self.alg.grad_sync(self.alg.optimizer.grad)
@@ -492,7 +489,7 @@ class ImpalaEngine(object):
         if self.train_net is not None and self._host_slab_plan() is not None:
             return self._learn_from_host_slabs(host, acts, bl, rew, dones, learning_rate, entropy_coeff)
         if self.train_net is not None:
-            # native learner: stacked uint8 observations -> conv1's space-to-depth input -> tcgen05 forward/backward
+            # native learner: stacked uint8 observations -> conv1's space-to-depth input -> wgmma forward/backward
             net = self.train_net
             slab = 16384
             for s0 in range(0, B * T, slab):

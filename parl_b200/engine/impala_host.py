@@ -1,4 +1,4 @@
-"""The IMPALA example's Actor and Agent on the B200, behind the reference's host contract — drop-in replacements
+"""The IMPALA example's Actor and Agent on the H100, behind the reference's host contract — drop-in replacements
 of examples/IMPALA/actor.py:27-105 and examples/IMPALA/atari_agent.py:21-74 for the Learner loop of
 examples/IMPALA/train.py:34-252:
 
@@ -13,7 +13,7 @@ examples/IMPALA/train.py:34-252:
 (one remote actor = one device actor pool instead of one CPU job with 5 envs); ``sample()`` runs the T-step rollout
 on the actor's own CUDA stream and copies the sample dict — keys / dtypes / env-major order of actor.py:79-91 — into
 pinned host memory (two alternating buffer sets: the dict handed out stays valid until the sample after next).
-``AtariAgent.learn`` uploads the numpy arrays and runs IMPALA.learn with the network on the tcgen05 kernels.
+``AtariAgent.learn`` uploads the numpy arrays and runs IMPALA.learn with the network on the wgmma kernels.
 """
 import os
 import time

@@ -21,7 +21,7 @@ class FlatAdam(object):
         assert len(self.params) > 0
         dev = self.params[0].device
         if dev.type != 'cuda':
-            raise RuntimeError('FlatAdam runs on the B200 only: move the model to CUDA first (no CPU fallback)')
+            raise RuntimeError('FlatAdam runs on the H100 only: move the model to CUDA first (no CPU fallback)')
         offs, total = [], 0
         for p in self.params:
             assert p.dtype == torch.float32 and p.device == dev

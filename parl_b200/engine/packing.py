@@ -1,6 +1,6 @@
 """Operand copies of the network kernels and their one-launch refresh.
 
-The tcgen05 kernels read the weights in their own layouts (bf16 KRSC filters, space-to-depth and transposed forms,
+The wgmma kernels read the weights in their own layouts (bf16 KRSC filters, space-to-depth and transposed forms,
 (H,W,C)-ordered fc columns, float32 biases).  Every element of every copy is ONE element of the optimizer's flat
 float32 master buffer (``FlatAdam.flat``; zero for padding), so after a learner update all of them are rebuilt by one
 ``rl_gather_cast`` launch per dtype from a precomputed index permutation — instead of ~26 permute + copy launches, which

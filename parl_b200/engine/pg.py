@@ -1,4 +1,4 @@
-"""REINFORCE on one B200 — the on-device replacement of benchmark/torch/QuickStart/train.py:28-76 (BASELINE
+"""REINFORCE on one H100 — the on-device replacement of benchmark/torch/QuickStart/train.py:28-76 (BASELINE
 configs[0]: CartPole policy gradient; the reference runs ONE env in one CPU process, here B envs run in lock-step).
 
     rollout  ONE launch (rl_rollout_mlp): T steps of CartPole physics + policy forward + exact categorical sampling

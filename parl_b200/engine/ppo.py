@@ -1,4 +1,4 @@
-"""PPO on one B200 — the on-device replacement of benchmark/torch/ppo/{train.py:45-126, agent.py:21-96,
+"""PPO on one H100 — the on-device replacement of benchmark/torch/ppo/{train.py:45-126, agent.py:21-96,
 storage.py:18-76, env_utils.py:28-117} (BASELINE configs[3]: MuJoCo-shaped continuous control, obs 17 / act 6,
 2048 envs x 2048 steps, 32 minibatches x 10 epochs, clipped-surrogate kernel).
 

@@ -1,4 +1,4 @@
-"""Learner-side forward AND backward of the Atari actor-critic on hand-written tcgen05 kernels — no autograd,
+"""Learner-side forward AND backward of the Atari actor-critic on hand-written wgmma kernels — no autograd,
 no cuDNN on the convolution path.
 
 Layers (a13: benchmark/torch/a2c/atari_model.py:23-96), all stride-1 in TMA-window form after space-to-depth:
@@ -7,8 +7,8 @@ Layers (a13: benchmark/torch/a2c/atari_model.py:23-96), all stride-1 in TMA-wind
 Backward (after the fused loss kernel delivered d_logits / d_values):
     heads/fc data gradients : rl_gemm_bf16_tn_masked (ReLU masks fused in the epilogue)
     conv data gradients     : rl_conv2d_s1_nhwc_bf16_dgrad (same windows, flipped taps, ReLU mask fused)
-    conv weight gradients   : rl_conv2d_s1_nhwc_bf16_wgrad (positions as the GEMM K dimension, TMEM-resident)
-    bias gradients          : from the weight-gradient pass (one extra tcgen05.mma per K step against ones); fc: rl_colsum_bf16
+    conv weight gradients   : rl_conv2d_s1_nhwc_bf16_wgrad (positions as the GEMM K dimension, register-resident accumulators)
+    bias gradients          : from the weight-gradient pass (one extra wgmma.mma per K step against ones); fc: rl_colsum_bf16
     fc / head weight gradients: two plain library GEMMs (torch.matmul -> cuBLAS), the only library calls left
 Activations for the whole learner batch stay resident in HBM (about 120 KB per sample in bf16).
 Gradients are written into the parameters' ``.grad`` views of the FlatAdam buffer in the reference layouts.
@@ -57,8 +57,8 @@ class AtariTrainNet(object):
         self.dw2 = torch.empty((64, 512), dtype=f32, device=dev)
         self.dw3 = torch.empty((64, 576), dtype=f32, device=dev)
         self.dbs = [torch.empty(n, dtype=f32, device=dev) for n in (512, 64, 64, 32)]     # bias-gradient scratch
-        # the two big fc contractions (K=5184 / N=5184 over all samples): our single-tile tcgen05 GEMM is L2-bound
-        # at this size, so by default they go to the library GEMM with our fused epilogue kernels around it
+        # the two big fc contractions (K=5184 / N=5184 over all samples) go to the library GEMM by default at large
+        # batches, with our fused epilogue kernels around it
         self.fc_library = fc_backend == 'library' or (fc_backend == 'auto' and N > 16384)
         self.da3c = e(N, 5184) if self.fc_library else None
         self.pack()

@@ -32,13 +32,13 @@ def add_graph_launches(n):
 
 
 def set_shiftconv_form(form):
-    """0 (default): one MMA group per filter tap; 1: column-tap-fused TMA-window conv tiles (measured slower; kept as
-    an experiment and cross-check)."""
+    """0 (default): one MMA chain per filter tap; 1: per filter column, the column shift applied to the output rows
+    (a cross-check of the tap / shift bookkeeping)."""
     _lib.check_config(_lib.load().rl_debug_set_shiftconv_form(int(form)), 'debug_set_shiftconv_form')
 
 
 def set_gemm_cluster(enable):
-    """1 (default): 2 x 2 cluster + TMA multicast form of rl_gemm_bf16_tn where the output has >= 2 x 2 wide tiles."""
+    """GEMM tile form: only the single-CTA form (enable=False) is built for sm_90a."""
     _lib.check_config(_lib.load().rl_debug_set_gemm_cluster(1 if enable else 0), 'debug_set_gemm_cluster')
 
 
@@ -541,7 +541,7 @@ def adam_step(param, grad, exp_avg, exp_avg_sq, lr, beta1, beta2, eps, step, gra
 
 # --------------------------------------------------------------------------- tensor-core contractions
 def gemm_bf16_tn(a, b, bias=None, relu=False, out_dtype=torch.bfloat16, out=None):
-    """C = act(a @ b.T + bias) on tcgen05 (rl_gemm_bf16_tn): a [M,K] bf16, b [N,K] bf16 (nn.Linear weight layout)."""
+    """C = act(a @ b.T + bias) on the tensor cores (rl_gemm_bf16_tn): a [M,K] bf16, b [N,K] bf16 (nn.Linear weight layout)."""
     require_cuda(a, b, bias)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and a.shape[1] == b.shape[1]
     M, K = a.shape
@@ -583,7 +583,7 @@ def gemm_bf16_tn_heads(a, b, bias, h_out, w2, b2, out2, relu=True):
 
 
 def conv2d_nhwc_bf16_fwd(x, weight_krsc, bias, KH, KW, stride, pad, relu=True, out=None):
-    """NHWC bf16 conv forward on tcgen05 (rl_conv2d_nhwc_bf16_fwd): x [N,H,W,Cin], weight [Cout, KH*KW*Cin] (r,s,c)."""
+    """NHWC bf16 conv forward on the tensor cores (rl_conv2d_nhwc_bf16_fwd): x [N,H,W,Cin], weight [Cout, KH*KW*Cin] (r,s,c)."""
     require_cuda(x, weight_krsc, bias)
     assert x.dtype == torch.bfloat16 and weight_krsc.dtype == torch.bfloat16 and bias.dtype == torch.float32
     N, H, W, Cin = x.shape
@@ -675,7 +675,7 @@ def colsum_bf16(x, out=None):
 
 
 def gemm_bf16_tn_masked(a, b, mask, out):
-    """out = (a @ b.T) * (mask > 0) on tcgen05 (rl_gemm_bf16_tn_masked); row strides of a / b / out / mask may
+    """out = (a @ b.T) * (mask > 0) on the tensor cores (rl_gemm_bf16_tn_masked); row strides of a / b / out / mask may
     exceed their widths (sub-matrix views)."""
     require_cuda(a, b)
     M, K = a.shape

@@ -1,7 +1,7 @@
 """``parl.connect`` façade (parl/remote/client.py:405-448).
 
 In the reference, connect() attaches the process to an xparl master that hands out CPU jobs.
-Here the "cluster" is the local B200(s): connect() records the address (kept only for logging /
+Here the "cluster" is the local H100(s): connect() records the address (kept only for logging /
 API compatibility), probes the visible devices and enables instantiation of ``@remote_class``
 objects, which are hosted in-process on the device actor pool — no ZeroMQ, no cloudpickle, no
 subprocesses.  Instantiating a remote class before connect() raises the reference's assertion."""

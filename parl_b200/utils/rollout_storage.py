@@ -1,5 +1,5 @@
 """``RolloutStorage`` in HBM — interface of benchmark/torch/ppo/storage.py:18-76 (append / compute_returns /
-sample_batch) with the (T,B) buffers resident on the B200: ``compute_returns`` is one launch of rl_gae_scan (the
+sample_batch) with the (T,B) buffers resident on the H100: ``compute_returns`` is one launch of rl_gae_scan (the
 reference's backward numpy loop, bit for bit in float32), ``sample_batch(idx)`` gathers the minibatch rows on the
 device (rl_gather_rows) and returns device tensors that ``PPO.learn`` takes as they are (numpy with ``as_numpy``)."""
 import numpy as np

@@ -1,6 +1,6 @@
 """``parl.utils.summary`` surface (parl/utils/summary.py:15-18, tensorboard.py:25-46): add_scalar /
 add_histogram / flush, lazily bound to tensorboardX when installed, otherwise a CSV file in the
-logger directory (tensorboardX is absent from the B200 image)."""
+logger directory (tensorboardX is absent from the H100 image)."""
 import os
 
 from .logger import logger

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the H100 box with -m gpu)')
     # make sure the C-ABI library matches the sources in the tree (no-op when the build stamp is current;
     # falls back to the prebuilt .so when no nvcc is available)
     from parl_b200.build import build

@@ -1,4 +1,4 @@
-"""BIT-EXACT checks of the tcgen05 network kernels on integer-valued operands.
+"""BIT-EXACT checks of the wgmma network kernels on integer-valued operands.
 
 bf16 tensor-core kernels cannot meet a 1e-4 tolerance against an fp32 network on generic data (the operands are
 rounded to 8 mantissa bits), so closeness tests alone cannot tell "right up to rounding" from "slightly wrong".  Here

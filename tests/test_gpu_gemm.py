@@ -1,4 +1,4 @@
-"""GPU parity: the tcgen05/TMA bf16 GEMM against a float32 torch matmul of the same bf16 inputs."""
+"""GPU parity: the wgmma/TMA bf16 GEMM against a float32 torch matmul of the same bf16 inputs."""
 import pytest
 import torch
 
@@ -29,7 +29,7 @@ def test_gemm_bf16_tn(M, N, K, relu):
                                                         (7, 11, 64, 64, 3, 1, 0), (300, 11, 64, 64, 3, 1, 0),
                                                         (64, 20, 32, 64, 4, 2, 2)])
 def test_conv2d_nhwc_bf16_fwd(N, H, Cin, Cout, k, stride, pad):
-    """tcgen05 implicit-GEMM conv vs torch conv2d in float32 on the same bf16 operands (the three layer shapes of
+    """wgmma implicit-GEMM conv vs torch conv2d in float32 on the same bf16 operands (the three layer shapes of
     the Atari actor-critic: s2d conv1, conv2 with padding, conv3)."""
     from parl_b200 import kernels as K_
     g = torch.Generator(device=DEV).manual_seed(N + H + Cin)
@@ -47,7 +47,7 @@ def test_conv2d_nhwc_bf16_fwd(N, H, Cin, Cout, k, stride, pad):
 
 @pytest.mark.parametrize('window_form', [True, False])
 def test_native_actor_net_matches_torch_model(window_form):
-    """The tcgen05 inference path (s2d conv1 -> conv2 -> conv3 -> fc -> policy head) against the torch model
+    """The wgmma inference path (s2d conv1 -> conv2 -> conv3 -> fc -> policy head) against the torch model
     (bf16 autocast) on real observations from the device env pool."""
     from parl_b200 import kernels as K_
     from parl_b200.engine.nets import AtariActorCritic
@@ -154,9 +154,9 @@ def test_conv2d_s1_dgrad_tma_window_form(N, H, Cin, Cout, k):
                                             (7, 21, 64, 32, 2), (160, 21, 64, 32, 2)])
 @pytest.mark.parametrize('legacy', [0, 2])
 def test_conv2d_s1_wgrad_tma_window_form(N, H, Cin, Cout, k, legacy):
-    """Window-form weight gradient (positions as the GEMM K dimension, MN-major tcgen05 operands) against torch
-    autograd on the same bf16 operands.  legacy=0: paired-tap M=128 form (two taps per instruction through the
-    descriptor's leading byte offset); legacy=2: one tap per M=64 instruction (Cout=32: role-swapped SWIZZLE_64B)."""
+    """Window-form weight gradient (positions as the GEMM K dimension, MN-major wgmma operands) against torch
+    autograd on the same bf16 operands.  legacy=0: A = input window, B = dout (Cout=32: SWIZZLE_64B), bias gradient
+    in the same pass; legacy=2: operand roles swapped for Cout=64, bias gradient by a column-sum pass."""
     from parl_b200 import kernels as K_, _lib
     _lib.load().rl_debug_set_wgrad_lane_map(legacy)
     try:
@@ -183,6 +183,30 @@ def _wgrad_case(K_, N, H, Cin, Cout, k):
     ref_db = dgrid.float().sum((0, 1, 2))
     assert (db - ref_db).abs().max().item() < 1e-2
     assert (dbf - ref_db).abs().max().item() < 1e-3 * max(1.0, ref_db.abs().max().item())   # fused bias gradient
+
+
+@pytest.mark.parametrize('N,H,Cin,Cout,k', [(160, 12, 128, 64, 2), (160, 11, 64, 64, 3), (160, 21, 64, 32, 2)])
+@pytest.mark.parametrize('legacy', [0, 2])
+def test_conv2d_s1_wgrad_without_bias_gradient(N, H, Cin, Cout, k, legacy):
+    """db=None changes how the accumulator slots are grouped: the workspace the library reports must still cover a
+    full grid of CTAs (more position tiles than SMs), in both weight-gradient forms."""
+    from parl_b200 import kernels as K_, _lib
+    g = torch.Generator(device=DEV).manual_seed(N + H + Cin)
+    Ho = H - k + 1
+    x = torch.randn(N, H, H, Cin, device=DEV, generator=g).to(torch.bfloat16)
+    dout = torch.randn(N, Ho, Ho, Cout, device=DEV, generator=g).to(torch.bfloat16)
+    w = torch.zeros(Cout, Cin, k, k, device=DEV, requires_grad=True)
+    torch.nn.functional.conv2d(x.float().permute(0, 3, 1, 2), w).backward(dout.float().permute(0, 3, 1, 2))
+    ref = w.grad.permute(0, 2, 3, 1).reshape(Cout, -1)
+    dgrid = torch.zeros(N, H, H, Cout, device=DEV, dtype=torch.bfloat16)
+    dgrid[:, :Ho, :Ho] = dout
+    _lib.load().rl_debug_set_wgrad_lane_map(legacy)
+    try:
+        dw = K_.conv2d_s1_nhwc_bf16_wgrad(dgrid, x, k, k)
+        torch.cuda.synchronize()
+    finally:
+        _lib.load().rl_debug_set_wgrad_lane_map(0)
+    assert (dw - ref).abs().max().item() < 1e-3 * max(1.0, ref.abs().max().item())
 
 
 def test_conv2d_s1_wgrad_accumulate_and_bias():
@@ -222,7 +246,7 @@ def test_obs_gather_s2d_matches_reference_layout():
 @pytest.mark.parametrize('M', [96, 512, 4096])
 def test_gemm_heads_fused_matches_separate_calls(M, heads_mma):
     """rl_gemm_bf16_tn_heads (actor fc + policy head; split-K reduce and heads in one kernel at small M) against the
-    two separate tcgen05 GEMMs for H (bit-identical) and an fp32 product of the stored bf16 H for the heads."""
+    two separate wgmma GEMMs for H (bit-identical) and an fp32 product of the stored bf16 H for the heads."""
     from parl_b200 import kernels as K_
     torch.manual_seed(M)
     N, Kd, N2 = 512, 5184, 18

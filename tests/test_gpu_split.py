@@ -1,4 +1,4 @@
-"""fp32-level verification of the tcgen05 kernels with float32 outputs (VERDICT r1 "pin network parity properly").
+"""fp32-level verification of the wgmma kernels with float32 outputs (VERDICT r1 "pin network parity properly").
 
 bf16 operands cannot meet 1e-4 against an fp32 network on generic data, which leaves the question whether the kernels
 are RIGHT or merely as noisy as autocast.  Here every fp32 operand is split into two bf16 pieces, x = hi + lo with

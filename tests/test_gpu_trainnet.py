@@ -1,4 +1,4 @@
-"""GPU parity: the hand-written learner network (AtariTrainNet: tcgen05 forward, dgrad, wgrad) against torch
+"""GPU parity: the hand-written learner network (AtariTrainNet: wgmma forward, dgrad, wgrad) against torch
 autograd through the same model (bf16 autocast), and the engine's native learn() against its autograd learn()."""
 import numpy as np
 import pytest

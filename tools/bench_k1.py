@@ -1,6 +1,6 @@
 """K1 (rl_vtrace_loss_fwd_bwd) timing matrix: kernel path x shape, two timing methods.
     python tools/bench_k1.py
- a) 'rot':   64 back-to-back launches over 8 rotating buffer sets (8 x 47 MB > 126 MB L2), captured in one CUDA graph,
+ a) 'rot':   64 back-to-back launches over 8 rotating buffer sets (8 x 47 MB > the 50 MB L2 of an H100), captured in one CUDA graph,
              one event pair around the replay (the eager Python loop next to it: host-launch-rate bound)
  b) 'flush': one event pair per launch, a 256 MB fill between launches evicts L2
 """
@@ -40,7 +40,9 @@ def flushed(T, B, A, n=12):
 
 if __name__ == '__main__':
     lib = _lib.load()
-    peak = 6571.6
+    # HBM peak: MEASURED_PEAKS.json at the repository root when present, else the H100 SXM data sheet (not measured)
+    peaks = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'MEASURED_PEAKS.json')
+    peak = float(json.load(open(peaks))['hbm_gbs']) if os.path.exists(peaks) else 3350.0
     for (T, B, A) in [(50, 4096, 18), (50, 512, 18), (50, 65536, 18)]:
         for mode in (0, 4, 9):
             lib.rl_debug_set_vtrace_path(mode)

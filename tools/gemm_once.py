@@ -1,5 +1,5 @@
-"""One launch of rl_gemm_bf16_tn per (shape, form) for ncu: the actor's and the learner's fc forward shapes, single-CTA
-and 2x2-cluster multicast forms.  python tools/gemm_once.py"""
+"""One launch of rl_gemm_bf16_tn per shape (for a profiler capture): the actor's and the learner's fc forward shapes.
+    python tools/gemm_once.py"""
 import sys
 
 import torch
@@ -15,9 +15,6 @@ for M, N, Kd in [(4096, 512, 5184), (204800, 512, 5184)]:
     b = (torch.randn(N, Kd, device=dev) * 0.1).to(bf)
     bias = torch.randn(N, device=dev)
     o = torch.empty(M, N, device=dev, dtype=bf)
-    for cl in (0, 1):
-        K.set_gemm_cluster(cl)
-        K.gemm_bf16_tn(a, b, bias, relu=True, out=o)
-        torch.cuda.synchronize()
-K.set_gemm_cluster(1)
+    K.gemm_bf16_tn(a, b, bias, relu=True, out=o)
+    torch.cuda.synchronize()
 print('done')
