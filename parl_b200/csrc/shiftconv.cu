@@ -211,9 +211,22 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
           const int yp = y + 2, xp = x + 2;
           obase = (((size_t)n * 12 + (yp >> 1)) * 12 + (xp >> 1)) * (4 * COUT) + (size_t)(((yp & 1) * 2 + (xp & 1)) * COUT);
         }
+        // ReLU-backward mask words, requested in groups of MJ before the group's first store, so that their load
+        // latencies overlap (a word loaded next to the store that consumes it is not hoisted past the preceding stores
+        // and per-element branches).  Cout <= 64: the whole row.  Cout = 128: the two accumulator halves leave room for
+        // 4 live words next to the 2x2 filter's state and 2 next to the 3x3 one's without adding spills.
+        constexpr int MJ = COUT <= 64 ? COUT / 8 : (KS == 2 ? 4 : 2);
 #pragma unroll
-        for (int j = 0; j < COUT / 8; ++j) {
-          const int i = 4 * j + 2 * rr, col = gmma_col(t, i);
+        for (int j0 = 0; j0 < COUT / 8; j0 += MJ) {
+        uint32_t mw[MJ];
+        if (has_mask && q < g.Q) {
+#pragma unroll
+          for (int jj = 0; jj < MJ; ++jj)
+            mw[jj] = __ldg(reinterpret_cast<const unsigned int*>(g.mask + (size_t)q * COUT + gmma_col(t, 4 * (j0 + jj) + 2 * rr)));
+        }
+#pragma unroll
+        for (int jj = 0; jj < MJ; ++jj) {
+          const int j = j0 + jj, i = 4 * j + 2 * rr, col = gmma_col(t, i);
           bool ok = valid;
           size_t dst_off = obase + col;
           if (g.out_mode == 2) {
@@ -231,11 +244,11 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
             pk = s_pack_bf16x2(d[h][i], d[h][i + 1]);
             if (has_mask) {
               // ReLU backward: keep the gradient where the saved activation is > 0 — one packed bf16x2 compare
-              const uint32_t mw = __ldg(reinterpret_cast<const unsigned int*>(g.mask + (size_t)q * COUT + col));
-              pk &= __hgt2_mask(*reinterpret_cast<const __nv_bfloat162*>(&mw), __floats2bfloat162_rn(0.f, 0.f));
+              pk &= __hgt2_mask(*reinterpret_cast<const __nv_bfloat162*>(&mw[jj]), __floats2bfloat162_rn(0.f, 0.f));
             }
           }
           *reinterpret_cast<uint32_t*>(g.out + dst_off) = pk;
+        }
         }
       }
     }
