@@ -32,9 +32,8 @@ int pdl_enabled();                   // 1: chain kernels are launched with progr
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // Opt a kernel in to the device's whole dynamic shared-memory range (227 KB minus its static use) ONCE per
-// device and never lower it again: the per-launch size is then free to vary between streams (actor: deep
-// pipelines, learner: shallower ones that leave L1 for the mask reads) without re-programming the function
-// while another launch of it is still queued.
+// device and never lower it again: the per-launch size is then free to vary with the launch's shapes without
+// re-programming the function while another launch of it is still queued.
 template <class Kernel>
 static inline void opt_in_max_dynamic_smem(Kernel kernel, unsigned long long* done_mask) {
   int dev = 0;

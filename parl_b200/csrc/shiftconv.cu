@@ -12,10 +12,14 @@
 //   conv1  8x8/4/p1, 4->32   == 2x2/1 on [21,21,64]   -> [20,20,32] written as s2d2-padded [12,12,128]
 //   conv2  4x4/2/p2, 32->64  == 2x2/1 on [12,12,128]  -> [11,11,64]
 //   conv3  3x3/1,    64->64  == 3x3/1 on [11,11,64]   -> [9,9,64]
-// Roles: warp 0 TMA producer (window ring); consumer warpgroups 1 and 2 take alternate tiles of the CTA (weights
-// resident in smem): each issues the tile's wgmma m64nCOUT chains for both 64-row halves into two register
-// accumulators, frees the window slot once they retire, and runs the epilogue (bias, ReLU or ReLU-backward mask,
-// bf16, layout-aware store) from its registers — one warpgroup's epilogue overlaps the other's MMAs.
+// Roles: warp 0 TMA producer (window ring; the data gradient's ring stage also holds the tile's ReLU mask, rows
+// [128 tile, 128 tile + 128) of the saved activation, loaded with the window); consumer warpgroups 1 and 2 take
+// alternate tiles of the CTA (weights resident in smem): each issues the tile's wgmma m64nCOUT chains for both 64-row
+// halves into two register accumulators and runs the epilogue — one warpgroup's epilogue overlaps the other's MMAs.
+// Forward: frees the window slot once the MMAs retire, then bias, ReLU, bf16 and layout-aware stores from the
+// registers.  Data gradient: stmatrix of the bf16 tile over its mask, ANDed with the mask words that ldmatrix reads
+// from the same place, then 16-byte chunks read back by consecutive threads, the ring stage freed, and the chunks
+// stored as contiguous destination runs.
 #include <cuda_bf16.h>
 
 #include "common.cuh"
@@ -28,6 +32,7 @@ namespace rl {
 constexpr int kScBM = 128;
 constexpr int kScMaxStages = 8;      // window ring depth is chosen at launch from the shared memory left by the weights
 constexpr int kScThreads = 384;      // producer warpgroup (warp 0 active) + 2 consumer warpgroups
+constexpr int kScEpiBar = 1;         // named barriers kScEpiBar + c: the epilogue of consumer warpgroup c (128 threads)
 
 struct ShiftConvArgs {
   const float* bias;
@@ -59,15 +64,29 @@ __device__ __forceinline__ uint32_t s_pack_relu_bf16x2(float lo, float hi) {
   return d;
 }
 
+// Byte offset of 16-byte chunk `ch` (columns 8ch .. 8ch + 7) of row `row` in a 128-row bf16 tile of the data gradient:
+// 64-column blocks of 128-byte rows, 16 KB apart, in the SWIZZLE_128B layout that a TMA load of the saved activation
+// writes (chunk ^ row % 8).  The 8 rows of one stmatrix / ldmatrix matrix, and 8 consecutive chunks of the copy-out,
+// fall on distinct banks.
+__device__ __forceinline__ uint32_t sc_tile_off(int row, int ch) {
+  return (uint32_t)((ch >> 3) * (kScBM * 128) + row * 128 + (((ch & 7) ^ (row & 7)) << 4));
+}
+
 // MODE 0: forward  (out = act(acc + bias), ReLU optional)     MODE 1: data gradient (out = acc * (mask > 0), mask optional)
 // U8IN (conv1 on the uint8 observation): map_in is the uint8 [Q][64] matrix, the producer fills a dense staging
 // ring and 256 more threads convert each window into the bf16 SWIZZLE_128B ring (u8win.cuh).
+// map_mask (MODE 1 with a mask): the saved activation [Q, COUT], 64-column x 128-row SWIZZLE_128B boxes.
+// The forward stores from the accumulator registers.  The data gradient stages its bf16 tile in shared memory and
+// writes it in 16-byte chunks; the forward does not: staging made conv3's MMA-bound forward (N = 64, 3x3) 10-15% and
+// the uint8 conv1 forward at the actor batch about 10% slower (H100 80GB HBM3, 400 W).
 template <int COUT, int CBLK, int KS, int MODE, bool U8IN = false>
 __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1)
     shiftconv_fwd_kernel(const __grid_constant__ CUtensorMap map_in, const __grid_constant__ CUtensorMap map_w,
-                         const ShiftConvArgs g) {
+                         const __grid_constant__ CUtensorMap map_mask, const ShiftConvArgs g) {
   static_assert(!U8IN || CBLK == 1, "the uint8 window is one 64-channel block");
+  static_assert(MODE == 0 || COUT % 64 == 0, "the data gradient's tile is made of 64-column mask boxes");
   constexpr int W_KB = COUT * 128;                        // one 64-wide weight k-block
+  constexpr int OUT_BYTES = kScBM * COUT * 2;             // one bf16 data-gradient tile
   extern __shared__ __align__(1024) unsigned char smem_dyn[];
   unsigned char* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   constexpr int num_kb = KS * KS * CBLK;                  // square KS x KS filter
@@ -78,14 +97,17 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
   __shared__ __align__(8) unsigned long long u8_full[kU8Stages], u8_empty[kU8Stages];
   const uint32_t nstages = (uint32_t)g.stages;
   unsigned char* sStage = sWin + nstages * CBLK * win_bytes;       // U8IN: [kU8Stages][wrows][64 B]
+  unsigned char* sOut = sWin + nstages * CBLK * win_bytes;         // MODE 1: [stages][OUT_BYTES] mask / output tiles
+  const bool has_mask = MODE == 1 && g.mask != nullptr;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_in);
     tma_prefetch_desc(&map_w);
+    if (has_mask) tma_prefetch_desc(&map_mask);
     for (int s = 0; s < kScMaxStages; ++s) {
       mbar_init(&full_bar[s], U8IN ? kU8Threads : 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], MODE == 0 ? 1 : 128);   // data gradient: every consumer thread, after its copy-out reads
     }
     for (int s = 0; s < kU8Stages; ++s) {
       mbar_init(&u8_full[s], 1);
@@ -117,12 +139,19 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
           if (++s == kU8Stages) s = 0, par ^= 1u;
         }
       } else {
+        const uint32_t tx = (uint32_t)(CBLK * g.wrows * 128) + (has_mask ? (uint32_t)OUT_BYTES : 0u);
         for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
           mbar_wait(&empty_bar[s], par);
-          mbar_arrive_expect_tx(&full_bar[s], (uint32_t)(CBLK * g.wrows * 128));
+          mbar_arrive_expect_tx(&full_bar[s], tx);
 #pragma unroll
           for (int cb = 0; cb < CBLK; ++cb)
             tma_load_2d(sWin + (s * CBLK + cb) * win_bytes, &map_in, cb * 64, tile * kScBM + g.row_shift, &full_bar[s]);
+          if (has_mask) {
+            // rows past Q of the last tile are zero-filled (and never stored)
+#pragma unroll
+            for (int cb = 0; cb < COUT / 64; ++cb)
+              tma_load_2d(sOut + s * OUT_BYTES + cb * (kScBM * 128), &map_mask, cb * 64, tile * kScBM, &full_bar[s]);
+          }
           if (++s == nstages) s = 0, par ^= 1u;
         }
       }
@@ -165,8 +194,13 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
     for (int i = 0; i < COUT / 2; ++i) bias_r[i] = __ldg(g.bias + gmma_col(t, i));
   }
   const bool relu = g.relu != 0;
-  const bool has_mask = MODE == 1 && g.mask != nullptr;
   const int HW = g.H * g.W;
+  constexpr int CH = COUT / 8;                      // 16-byte chunks of an output row
+  // stmatrix / ldmatrix: lane l addresses row l % 8 of matrix l / 8 = (row half (l / 8) % 2, chunk j + l / 16)
+  const int mx_row = 16 * (t >> 5) + (lane & 7) + 8 * ((lane >> 3) & 1), mx_ch = lane >> 4;
+  // copy-out: thread t moves chunk t % CH of rows t / CH + RSTEP k, consecutive threads cover a row's chunks in order
+  constexpr int RSTEP = kScBM / CH;
+  const int cp_ch = t % CH, cp_row = t / CH;
   uint32_t s = (uint32_t)c, full_par = 0;
   for (long long tile = blockIdx.x + (long long)c * gridDim.x; tile < g.num_tiles; tile += 2 * gridDim.x) {
     float d[2][COUT / 2];                            // rows [0, 64) and [64, 128) of the tile
@@ -191,65 +225,91 @@ __global__ void __launch_bounds__(U8IN ? kScThreads + kU8Threads : kScThreads, 1
     wgmma_wait<0>();
     wgmma_fence_regs(d[0]);
     wgmma_fence_regs(d[1]);
-    if (t == 0) mbar_arrive(&empty_bar[s]);        // the window slot is free for the next TMA load
-    s += 2;
-    if (s >= nstages) s -= nstages, full_par ^= 1u;
+    if constexpr (MODE == 0) {
+      // forward: the window slot is free as soon as the MMAs retire; bias + ReLU, bf16, stored from the registers
+      if (t == 0) mbar_arrive(&empty_bar[s]);
+      s += 2;
+      if (s >= nstages) s -= nstages, full_par ^= 1u;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {               // the thread's two rows of this half: r0 and r0 + 8
-        const int q = (int)tile * kScBM + 64 * h + gmma_row(t, 2 * rr);
-        const int n = q / HW;
-        const int rem = q - n * HW;
-        const int y = rem / g.W, x = rem - y * g.W;
-        const bool valid = q < g.Q && y < g.Hout && x < g.Wout;
-        size_t obase = 0;
-        if (g.out_mode == 0) {
-          obase = ((size_t)(n * g.OGH + y) * g.OGW + x) * COUT;
-        } else if (g.out_mode == 1) {
-          // conv1 -> conv2 input: zero-padded by 2, 2x2 space-to-depth: [n, (y+2)/2, (x+2)/2, ((y&1)*2 + (x&1))*COUT + c]
-          const int yp = y + 2, xp = x + 2;
-          obase = (((size_t)n * 12 + (yp >> 1)) * 12 + (xp >> 1)) * (4 * COUT) + (size_t)(((yp & 1) * 2 + (xp & 1)) * COUT);
-        }
-        // ReLU-backward mask words, requested in groups of MJ before the group's first store, so that their load
-        // latencies overlap (a word loaded next to the store that consumes it is not hoisted past the preceding stores
-        // and per-element branches).  Cout <= 64: the whole row.  Cout = 128: the two accumulator halves leave room for
-        // 4 live words next to the 2x2 filter's state and 2 next to the 3x3 one's without adding spills.
-        constexpr int MJ = COUT <= 64 ? COUT / 8 : (KS == 2 ? 4 : 2);
-#pragma unroll
-        for (int j0 = 0; j0 < COUT / 8; j0 += MJ) {
-        uint32_t mw[MJ];
-        if (has_mask && q < g.Q) {
-#pragma unroll
-          for (int jj = 0; jj < MJ; ++jj)
-            mw[jj] = __ldg(reinterpret_cast<const unsigned int*>(g.mask + (size_t)q * COUT + gmma_col(t, 4 * (j0 + jj) + 2 * rr)));
-        }
-#pragma unroll
-        for (int jj = 0; jj < MJ; ++jj) {
-          const int j = j0 + jj, i = 4 * j + 2 * rr, col = gmma_col(t, i);
-          bool ok = valid;
-          size_t dst_off = obase + col;
-          if (g.out_mode == 2) {
-            // channel block (dy,dx) of position (Y,X) is pixel (2Y+dy-2, 2X+dx-2) of the 20x20 image, 32 channels
-            const int blk = col >> 5, py = 2 * y + (blk >> 1) - 2, px = 2 * x + (blk & 1) - 2;
-            ok = q < g.Q && py >= 0 && py < 20 && px >= 0 && px < 20;
-            dst_off = (((size_t)n * 21 + py) * 21 + px) * 32 + (col & 31);
-          }
-          if (!ok) continue;
-          uint32_t pk;
-          if (MODE == 0) {
-            const float v0 = d[h][i] + bias_r[i], v1 = d[h][i + 1] + bias_r[i + 1];
-            pk = relu ? s_pack_relu_bf16x2(v0, v1) : s_pack_bf16x2(v0, v1);
+        for (int rr = 0; rr < 2; ++rr) {             // the thread's two rows of this half: r0 and r0 + 8
+          const int q = (int)tile * kScBM + 64 * h + gmma_row(t, 2 * rr);
+          const int n = q / HW;
+          const int rem = q - n * HW;
+          const int y = rem / g.W, x = rem - y * g.W;
+          const bool valid = q < g.Q && y < g.Hout && x < g.Wout;
+          size_t obase;
+          if (g.out_mode == 0) {
+            obase = ((size_t)(n * g.OGH + y) * g.OGW + x) * COUT;
           } else {
-            pk = s_pack_bf16x2(d[h][i], d[h][i + 1]);
-            if (has_mask) {
-              // ReLU backward: keep the gradient where the saved activation is > 0 — one packed bf16x2 compare
-              pk &= __hgt2_mask(*reinterpret_cast<const __nv_bfloat162*>(&mw[jj]), __floats2bfloat162_rn(0.f, 0.f));
-            }
+            // conv1 -> conv2 input: zero-padded by 2, 2x2 space-to-depth: [n, (y+2)/2, (x+2)/2, ((y&1)*2 + (x&1))*COUT + c]
+            const int yp = y + 2, xp = x + 2;
+            obase = (((size_t)n * 12 + (yp >> 1)) * 12 + (xp >> 1)) * (4 * COUT) + (size_t)(((yp & 1) * 2 + (xp & 1)) * COUT);
           }
-          *reinterpret_cast<uint32_t*>(g.out + dst_off) = pk;
+#pragma unroll
+          for (int j = 0; j < CH; ++j) {
+            const int i = 4 * j + 2 * rr;
+            if (!valid) continue;
+            const float v0 = d[h][i] + bias_r[i], v1 = d[h][i + 1] + bias_r[i + 1];
+            *reinterpret_cast<uint32_t*>(g.out + obase + gmma_col(t, i)) =
+                relu ? s_pack_relu_bf16x2(v0, v1) : s_pack_bf16x2(v0, v1);
+          }
         }
+      }
+    } else {
+      // data gradient: the bf16 tile is staged over the tile's mask (or in the mask slot), then copied out
+      const unsigned char* tile_p = sOut + s * OUT_BYTES;
+      const uint32_t otile = smem_u32(tile_p);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int j = 0; j < CH; j += 2) {
+          uint32_t pk[4];                            // matrix m = (row half m % 2, chunk j + m / 2): elements 4j + 2m, +1
+#pragma unroll
+          for (int m = 0; m < 4; ++m) pk[m] = s_pack_bf16x2(d[h][4 * j + 2 * m], d[h][4 * j + 2 * m + 1]);
+          const uint32_t a = otile + sc_tile_off(64 * h + mx_row, j + mx_ch);
+          if (has_mask) {
+            // ReLU backward: keep the gradient where the saved activation is > 0 — one packed bf16x2 compare per word
+            uint32_t mw[4];
+            ldmatrix_x4(a, mw);
+#pragma unroll
+            for (int m = 0; m < 4; ++m)
+              pk[m] &= __hgt2_mask(*reinterpret_cast<const __nv_bfloat162*>(&mw[m]), __floats2bfloat162_rn(0.f, 0.f));
+          }
+          stmatrix_x4(a, pk);
         }
+      }
+      named_bar_sync(kScEpiBar + c, 128);            // the warpgroup's tile is staged
+      uint4 v[CH];
+#pragma unroll
+      for (int k = 0; k < CH; ++k) v[k] = *reinterpret_cast<const uint4*>(tile_p + sc_tile_off(cp_row + RSTEP * k, cp_ch));
+      fence_proxy_async_smem();                      // these generic accesses come before the next TMA write of the slot
+      mbar_arrive(&empty_bar[s]);                    // every thread: the window and the mask slot are free
+      s += 2;
+      if (s >= nstages) s -= nstages, full_par ^= 1u;
+      int q = (int)tile * kScBM + cp_row;
+      int n = q / HW;
+      int y = (q - n * HW) / g.W;
+      int x = q - n * HW - y * g.W;
+#pragma unroll
+      for (int k = 0; k < CH; ++k) {
+        const int col = 8 * cp_ch;
+        bool ok = q < g.Q;
+        size_t dst_off;
+        if (g.out_mode == 0) {
+          ok = ok && y < g.Hout && x < g.Wout;
+          dst_off = ((size_t)(n * g.OGH + y) * g.OGW + x) * COUT + col;
+        } else {
+          // channel block (dy,dx) of position (Y,X) is pixel (2Y+dy-2, 2X+dx-2) of the 20x20 image, 32 channels
+          const int blk = col >> 5, py = 2 * y + (blk >> 1) - 2, px = 2 * x + (blk & 1) - 2;
+          ok = ok && py >= 0 && py < 20 && px >= 0 && px < 20;
+          dst_off = (((size_t)n * 21 + py) * 21 + px) * 32 + (col & 31);
+        }
+        if (ok) *reinterpret_cast<uint4*>(g.out + dst_off) = v[k];
+        q += RSTEP;
+        for (x += RSTEP; x >= g.W; x -= g.W)
+          if (++y == g.H) y = 0, ++n;
       }
     }
   }
@@ -467,15 +527,16 @@ static int sc_make_map(CUtensorMap* map, const void* base, uint64_t cols, uint64
 static size_t u8_ring_bytes(int wrows) { return (size_t)kU8Stages * (size_t)((wrows * 64 + 1023) & ~1023); }
 
 template <int COUT, int CBLK, int KS, int MODE, bool U8IN = false>
-static void launch_shiftconv(const CUtensorMap& mi, const CUtensorMap& mw, const ShiftConvArgs& g, int num_kb, int sms,
-                             cudaStream_t st) {
+static void launch_shiftconv(const CUtensorMap& mi, const CUtensorMap& mw, const CUtensorMap& mm, const ShiftConvArgs& g,
+                             int num_kb, int sms, cudaStream_t st) {
   const size_t win = (size_t)((g.wrows * 128 + 1023) & ~1023);
-  const size_t smem = (size_t)((num_kb * COUT * 128 + 1023) & ~1023) + (size_t)g.stages * CBLK * win + 1024 +
+  const size_t tile = MODE == 1 ? (size_t)kScBM * COUT * 2 : 0;      // data gradient: mask / output tile per stage
+  const size_t smem = (size_t)((num_kb * COUT * 128 + 1023) & ~1023) + (size_t)g.stages * (CBLK * win + tile) + 1024 +
                       (U8IN ? u8_ring_bytes(g.wrows) : 0);
   auto kern = shiftconv_fwd_kernel<COUT, CBLK, KS, MODE, U8IN>;
   RL_SMEM_OPTIN(kern);
   const int grid = g.num_tiles < sms ? g.num_tiles : sms;
-  launch_chain(kern, dim3(grid), dim3(U8IN ? kScThreads + kU8Threads : kScThreads), smem, st, mi, mw, g);
+  launch_chain(kern, dim3(grid), dim3(U8IN ? kScThreads + kU8Threads : kScThreads), smem, st, mi, mw, mm, g);
 }
 
 template <int COUT, int CBLK, int KS, int MODE, bool U8IN = false>
@@ -537,21 +598,23 @@ static int shiftconv_launch(const void* in, const void* weight, const float* bia
   const size_t win = (size_t)((g.wrows * 128 + 1023) & ~1023);
   {
     const size_t acc = coltap ? (size_t)kScBM * Cout * sizeof(float) : 0;    // column-tap form: fp32 output tile
+    const size_t tile = transposed && !coltap ? (size_t)kScBM * Cout * 2 : 0;  // data gradient: mask / output tile
     const size_t budget = 220 * 1024 - ((size_t)num_kb * Cout * 128 + 2048) - (u8in ? u8_ring_bytes(g.wrows) : 0) - acc;
-    long long st = (long long)(budget / ((size_t)cblk * win));
+    long long st = (long long)(budget / ((size_t)cblk * win + tile));
     if (st > kScMaxStages) st = kScMaxStages;
-    // the dgrad epilogue reads the ReLU mask through L1: leave the unified L1/shared array some cache
-    if (mask && st > 4) st = 4;
     RL_CHECK_ARG(st >= 2, "%s: weights + windows do not fit in shared memory", name);
     g.stages = (int)st;
   }
-  alignas(64) CUtensorMap mi, mw;
+  alignas(64) CUtensorMap mi, mw, mm;
   if ((u8in ? make_tensor_map_u8_rows64(&mi, in, (uint64_t)Q, (uint32_t)g.wrows)
             : sc_make_map(&mi, in, (uint64_t)Cin, (uint64_t)Q, (uint32_t)g.wrows)) ||
-      sc_make_map(&mw, weight, (uint64_t)KH * KW * Cin, (uint64_t)Cout, (uint32_t)Cout)) {
+      sc_make_map(&mw, weight, (uint64_t)KH * KW * Cin, (uint64_t)Cout, (uint32_t)Cout) ||
+      // the ReLU mask of a tile: its 128 accumulator rows of the saved activation [Q, Cout]
+      (mask && !coltap && sc_make_map(&mm, mask, (uint64_t)Cout, (uint64_t)Q, (uint32_t)kScBM))) {
     set_error("%s: cuTensorMapEncodeTiled failed", name);
     return RL_ERR_CUDA;
   }
+  if (!mask || coltap) mm = mi;                 // not read
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -577,16 +640,16 @@ static int shiftconv_launch(const void* in, const void* weight, const float* bia
     }
   } else
   switch (key) {
-    case 1003212: launch_shiftconv<32, 1, 2, 0, true>(mi, mw, g, num_kb, sms, st); break;  // conv1 fwd, uint8 input
-    case 3212: launch_shiftconv<32, 1, 2, 0>(mi, mw, g, num_kb, sms, st); break;          // conv1 fwd
-    case 6422: launch_shiftconv<64, 2, 2, 0>(mi, mw, g, num_kb, sms, st); break;          // conv2 fwd
-    case 6413: launch_shiftconv<64, 1, 3, 0>(mi, mw, g, num_kb, sms, st); break;          // conv3 fwd
-    case 6412: launch_shiftconv<64, 1, 2, 0>(mi, mw, g, num_kb, sms, st); break;
-    case 6423: launch_shiftconv<64, 2, 3, 0>(mi, mw, g, num_kb, sms, st); break;
-    case 106413: launch_shiftconv<64, 1, 3, 1>(mi, mw, g, num_kb, sms, st); break;        // conv3 dgrad
-    case 112812: launch_shiftconv<128, 1, 2, 1>(mi, mw, g, num_kb, sms, st); break;       // conv2 dgrad
-    case 106412: launch_shiftconv<64, 1, 2, 1>(mi, mw, g, num_kb, sms, st); break;
-    case 112813: launch_shiftconv<128, 1, 3, 1>(mi, mw, g, num_kb, sms, st); break;
+    case 1003212: launch_shiftconv<32, 1, 2, 0, true>(mi, mw, mm, g, num_kb, sms, st); break;  // conv1 fwd, uint8 input
+    case 3212: launch_shiftconv<32, 1, 2, 0>(mi, mw, mm, g, num_kb, sms, st); break;          // conv1 fwd
+    case 6422: launch_shiftconv<64, 2, 2, 0>(mi, mw, mm, g, num_kb, sms, st); break;          // conv2 fwd
+    case 6413: launch_shiftconv<64, 1, 3, 0>(mi, mw, mm, g, num_kb, sms, st); break;          // conv3 fwd
+    case 6412: launch_shiftconv<64, 1, 2, 0>(mi, mw, mm, g, num_kb, sms, st); break;
+    case 6423: launch_shiftconv<64, 2, 3, 0>(mi, mw, mm, g, num_kb, sms, st); break;
+    case 106413: launch_shiftconv<64, 1, 3, 1>(mi, mw, mm, g, num_kb, sms, st); break;        // conv3 dgrad
+    case 112812: launch_shiftconv<128, 1, 2, 1>(mi, mw, mm, g, num_kb, sms, st); break;       // conv2 dgrad
+    case 106412: launch_shiftconv<64, 1, 2, 1>(mi, mw, mm, g, num_kb, sms, st); break;
+    case 112813: launch_shiftconv<128, 1, 3, 1>(mi, mw, mm, g, num_kb, sms, st); break;
     default:
       set_error("%s: no instantiation for Cout=%d Cin=%d %dx%d", name, Cout, Cin, KH, KW);
       return RL_ERR_BAD_ARG;

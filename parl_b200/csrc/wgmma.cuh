@@ -87,6 +87,21 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint6
 // row / column of accumulator element i (see the layout at the top) for warpgroup thread t
 __device__ __forceinline__ int gmma_row(int t, int i) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
 __device__ __forceinline__ int gmma_col(int t, int i) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
+
+// Four 8x8 b16 matrices between shared memory and registers.  Lane l gives the address of row l % 8 of matrix l / 8;
+// word m of lane l is row l / 4, columns 2 (l % 4) and 2 (l % 4) + 1 of matrix m, which is where an accumulator
+// packed to bf16x2 keeps (d[4j + 2rr], d[4j + 2rr + 1]) of one 8-row, 8-column block.
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];\n"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
 #endif
 
 }  // namespace rl

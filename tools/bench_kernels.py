@@ -1,5 +1,5 @@
 """Micro-benchmarks of individual kernels (CUDA events, rotating >L2 buffers).
-    python tools/bench_kernels.py [vtrace|env|losses|all]
+    python tools/bench_kernels.py [vtrace|env|losses|conv|all]     (conv is not part of all)
 """
 import json
 import sys
@@ -189,8 +189,65 @@ def bench_mlp(N=131072, dims=(17, 64, 64), heads=(6, 1)):
                 fwd_gbps=N * (dims[0] + sum(heads)) * 4 / sf / 1e9)
 
 
+# The five window-conv calls of the Atari actor-critic (engine/train_net.py):
+#   name, call, input [H,W,C] (and dtype), weight [rows, cols], output shape, out_mode, mask [H,W,C], bytes written per sample
+# Algorithmic bytes are what the layer has to move: its input, the ReLU mask of a data gradient, and the valid output
+# region it writes.  MMA FLOPs are what the kernel issues: every position of every 128-row tile, dropped ones included.
+_CONVS = (
+    ('conv1_fwd', 'fwd', (21, 21, 64), torch.uint8, (32, 256), (12, 12, 128), 1, None, 20 * 20 * 32 * 2),
+    ('conv2_fwd', 'fwd', (12, 12, 128), torch.bfloat16, (64, 512), (11, 11, 64), 0, None, 11 * 11 * 64 * 2),
+    ('conv3_fwd', 'fwd', (11, 11, 64), torch.bfloat16, (64, 576), (9, 9, 64), 0, None, 9 * 9 * 64 * 2),
+    ('conv3_dgrad', 'dgrad', (11, 11, 64), torch.bfloat16, (64, 576), (12, 12, 64), 0, (11, 11, 64), 11 * 11 * 64 * 2),
+    ('conv2_dgrad', 'dgrad', (12, 12, 64), torch.bfloat16, (128, 256), (21, 21, 32), 2, (12, 12, 128), 20 * 20 * 32 * 2),
+)
+_HBM_TBS, _BF16_TFLOPS = 3.35, 989.0      # H100 SXM data sheet (dense BF16)
+
+
+def bench_conv(name, N, nbuf, iters):
+    """One window-conv call (shiftconv_fwd_kernel) at batch N, timed with CUDA events over `nbuf` rotating operand sets."""
+    _, kind, xs, xdt, ws, os_, out_mode, ms_, out_bytes = next(c for c in _CONVS if c[0] == name)
+    dev = 'cuda:0'
+    g = torch.Generator(device=dev).manual_seed(7)
+    k = 3 if ws[1] == 576 else 2
+    w = (0.05 * torch.randn(ws, device=dev, generator=g)).to(torch.bfloat16)
+    bias = 0.1 * torch.randn(ws[0], device=dev, generator=g)
+    sets = []
+    for _ in range(nbuf):
+        if xdt == torch.uint8:
+            x = torch.randint(0, 256, (N, ) + xs, device=dev, dtype=torch.uint8, generator=g)
+        else:
+            x = torch.randn((N, ) + xs, device=dev, generator=g).to(torch.bfloat16)
+        mask = torch.randn((N, ) + ms_, device=dev, generator=g).to(torch.bfloat16) if ms_ else None
+        sets.append((x, mask, torch.zeros((N, ) + os_, device=dev, dtype=torch.bfloat16)))
+
+    def run(i):
+        x, mask, out = sets[i % nbuf]
+        if kind == 'fwd':
+            K.conv2d_s1_nhwc_bf16_fwd(x, w, bias, k, k, relu=True, out=out, out_mode=out_mode)
+        else:
+            K.conv2d_s1_nhwc_bf16_dgrad(x, w, k, k, out, act_mask=mask, out_mode=out_mode)
+    sec = time_fn(run, iters=iters, warmup=max(3, nbuf))
+    in_bytes = xs[0] * xs[1] * xs[2] * (1 if xdt == torch.uint8 else 2)
+    mask_bytes = ms_[0] * ms_[1] * ms_[2] * 2 if ms_ else 0
+    alg_bytes = N * (in_bytes + mask_bytes + out_bytes)
+    tiles = -(-N * xs[0] * xs[1] // 128)
+    mma_flop = 2.0 * tiles * 128 * ws[0] * ws[1]        # M = positions, N = output channels, K = taps x input channels
+    t_hbm, t_mma = alg_bytes / (_HBM_TBS * 1e12), mma_flop / (_BF16_TFLOPS * 1e12)
+    return dict(kernel=name, N=N, ms=sec * 1e3, alg_bytes=alg_bytes, mma_flop=mma_flop,
+                bound='hbm' if t_hbm >= t_mma else 'mma', bound_ms=max(t_hbm, t_mma) * 1e3,
+                share=max(t_hbm, t_mma) / sec, peaks='H100 SXM data sheet: 3.35 TB/s, 989 TFLOP/s dense BF16')
+
+
 if __name__ == '__main__':
     which = sys.argv[1] if len(sys.argv) > 1 else 'all'
+    if which == 'conv':
+        # learner batch: 50 steps x 4096 envs (operands far larger than the L2);  actor batch: 4096, rotating operand
+        # sets so that no call finds its input in the 50 MB L2
+        for name in [c[0] for c in _CONVS]:
+            print(json.dumps(bench_conv(name, 50 * 4096, nbuf=1, iters=10)))
+            torch.cuda.empty_cache()
+        for name in [c[0] for c in _CONVS]:
+            print(json.dumps(bench_conv(name, 4096, nbuf=4, iters=100)))
     if which == 'vtrace_cpasync':
         from parl_b200 import _lib
         _lib.load().rl_debug_set_tma(1)
