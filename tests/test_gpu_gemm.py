@@ -242,11 +242,25 @@ def test_obs_gather_s2d_matches_reference_layout():
     assert torch.equal(out, ref.to(torch.bfloat16))
 
 
+@pytest.fixture
+def sm_limit(request):
+    """CTA caps (rl_set_sm_limit) that change the GEMM's tile width and split-K choice; 57 is the pipelined engine's
+    actor cap.  0 (one CTA per SM) is restored afterwards."""
+    from parl_b200 import kernels as K_
+    K_.set_sm_limit(request.param)
+    try:
+        yield request.param
+    finally:
+        K_.set_sm_limit(0)
+
+
 @pytest.mark.parametrize('heads_mma', [1, 0])
-@pytest.mark.parametrize('M', [96, 512, 4096])
-def test_gemm_heads_fused_matches_separate_calls(M, heads_mma):
+@pytest.mark.parametrize('M,sm_limit', [pytest.param(M, k, id=str(M) if k == 0 else '%d-sms%d' % (M, k))
+                                        for M in (96, 512, 4096) for k in (0, 1, 2, 57, 75)], indirect=['sm_limit'])
+def test_gemm_heads_fused_matches_separate_calls(M, heads_mma, sm_limit):
     """rl_gemm_bf16_tn_heads (actor fc + policy head; split-K reduce and heads in one kernel at small M) against the
-    two separate wgmma GEMMs for H (bit-identical) and an fp32 product of the stored bf16 H for the heads."""
+    two separate wgmma GEMMs for H (bit-identical) and an fp32 product of the stored bf16 H for the heads, both under
+    the same CTA cap."""
     from parl_b200 import kernels as K_
     torch.manual_seed(M)
     N, Kd, N2 = 512, 5184, 18
