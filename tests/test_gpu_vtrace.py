@@ -139,7 +139,8 @@ def test_vtrace_loss_full_size_properties():
 def test_tma_and_cpasync_tile_paths_agree():
     """The TMA tensor-map tile path and the cp.async path of the general (v4) kernel are the same arithmetic, and
     the default v8 kernel (register-resident packed-pair arithmetic, two passes in time, in-warp scan) agrees with
-    both to float32 round-off (shapes v8 does not take — T > 64 — run v4 twice)."""
+    both to float32 round-off.  v8 takes int32 actions only, so modes 0 and 9 get them (shapes v8 does not take —
+    T > 64 — run v4 twice)."""
     from parl_b200 import kernels, _lib
     lib = _lib.load()
     for (T, B, A) in [(50, 512, 18), (50, 7 * 4, 6), (130, 64, 18), (20, 256, 2), (50, 4096, 18), (7, 8, 18),
@@ -147,6 +148,8 @@ def test_tma_and_cpasync_tile_paths_agree():
         tl, bl, acts, rew, dones, vals = make_rollout(T, B, A, 11)
         args = [_cuda(tl).reshape(T * B, A), _cuda(bl).reshape(T * B, A), _cuda(acts).reshape(-1),
                 _cuda(rew).reshape(-1), _cuda(dones).reshape(-1), _cuda(vals).reshape(-1)]
+        args32 = list(args)
+        args32[2] = args[2].to(torch.int32)
         try:
             lib.rl_debug_set_vtrace_path(4)
             lib.rl_debug_set_tma(1)
@@ -160,7 +163,7 @@ def test_tma_and_cpasync_tile_paths_agree():
             assert torch.equal(r0['losses'][:5], r1['losses'][:5])
             for mode in (0, 9):
                 lib.rl_debug_set_vtrace_path(mode)
-                r5 = kernels.vtrace_loss_fwd_bwd(*args, T, B, 0.99, 0.5, -0.01, want_returns=True)
+                r5 = kernels.vtrace_loss_fwd_bwd(*args32, T, B, 0.99, 0.5, -0.01, want_returns=True)
                 torch.cuda.synchronize()
                 for k in ('d_logits', 'd_values', 'vs', 'pg_advantages'):
                     assert torch.allclose(r5[k], r1[k], rtol=2e-5, atol=2e-5), (k, T, B, A, mode,
